@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — 1080p H.264 encode throughput of the B200 macroblock pipeline (BASELINE.json metric).
+"""bench.py — 1080p H.264 encode throughput of the H100 macroblock pipeline (BASELINE.json metric).
 
 A "step" = one batch-frame: every one of the S independent 1080p streams resident on this GPU advances by
 one picture (mode decision + ME + transform/quant + reconstruction + deblocking + border expansion on the
@@ -18,9 +18,13 @@ reference encoder (oracle/_ref) run on the same picture order: "parity_checked" 
 mismatch fails the run.  A second workload point ("workload_hard": +-8 noise, few skipped macroblocks, ~27x the bits) is reported
 next to the headline.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--streams S] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--streams S] [--impl reference] [--dump-outputs DIR]
 
-N > 1: one process per GPU under torch.distributed (launched by the driver with torchrun); streams are
+--dump-outputs DIR: after the timed steps, the access units the last timed step of the resident run returned (every
+stream, bytes as float32, concatenated) and their lengths and frame types go to DIR/*.npy; the inputs are seeded,
+so two builds run with the same arguments can be compared output for output.
+
+N > 1: one process per GPU under torch.distributed (launched with torchrun); streams are
 independent, there is no data-path collective ("scaling": "weak"); NCCL is used only for the barrier and the
 max-over-ranks of the timed interval.
 """
@@ -83,12 +87,12 @@ def host_cores():
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
-        return json.load(open(p)).get("hbm_gbs", 6650.0), "measured"
-    return 6650.0, "fallback"
+        return json.load(open(p)).get("hbm_gbs", 3350.0), "measured"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -228,14 +232,6 @@ def reference_hashes(clip, seq, n_pictures, classes):
     return out
 
 
-def ncu_traffic(kernel):
-    """per-launch DRAM bytes of `kernel` from the committed ncu capture (profiles/ncu_traffic.json), or None"""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json"))).get(kernel)
-    except Exception:
-        return None
-
-
 def mc_sad_roofline(L, local, peak):
     """BASELINE metric 2: the MC+SAD unit (b2h264_k_mc_sad, layer 1) against the HBM roofline.  64 stacked 1080p
     planes (cur + padded ref = 302 MB, larger than L2); algorithmic bytes per MB = 256 cur + 256 ref + 4 K vector +
@@ -277,10 +273,8 @@ def mc_sad_roofline(L, local, peak):
         gbs = n * alg / sec / 1e9
         out[name] = {"achieved": gbs, "frac": gbs / peak, "us_per_launch": sec * 1e6, "mb_per_launch": n, "candidates_per_mb": k,
                      "alg_bytes_per_mb": alg}
-    t = ncu_traffic("k_mc_sad_tma")
     return {"kernel": "k_mc_sad_tma (b2h264_k_mc_sad: 8x4-MB tiles staged by TMA bulk tensor copies, separable half-sample planes per tile)",
             "bound": "hbm", "unit": "GB/s",
-            "traffic": t["dram_bytes"] if t and t.get("mb_per_launch") == n else None,
             "peak": peak, "alg_bytes_per_mb": 520, "candidates_per_mb": 1, "achieved": out["integer"]["achieved"],
             "frac": out["integer"]["frac"], "integer_mv": out["integer"], "quarter_pel_mv": out["quarter"], "mixed_9_candidates": out["mixed9"],
             "note": "64 stacked padded 1080p planes per launch (302 MB of pixels, larger than L2)"}
@@ -349,6 +343,17 @@ def api_run(args, local, clip_path, out_prefix, S):
     return res
 
 
+def dump_outputs(out_dir, aus, frame_types):
+    """the access units of one step: their bytes concatenated in stream order as float32 (the leading streams whose units
+    fit 60 MB: all 256 of the default workload, ~5 KB each), and the lengths and frame types of every stream"""
+    os.makedirs(out_dir, exist_ok=True)
+    n = int(np.searchsorted(np.cumsum([len(a) for a in aus]), (60 << 20) // 4, side="right"))
+    data = np.frombuffer(b"".join(bytes(a) for a in aus[:n]), np.uint8)
+    np.save(os.path.join(out_dir, "access_units.npy"), data.astype(np.float32))
+    np.save(os.path.join(out_dir, "access_unit_bytes.npy"), np.array([len(a) for a in aus], np.float32))
+    np.save(os.path.join(out_dir, "frame_types.npy"), np.array(frame_types, np.float32))
+
+
 # ---------------------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -363,6 +368,7 @@ def main():
     ap.add_argument("--no-api", action="store_true", help="skip the run through ISVCEncoder::EncodeFrame")
     ap.add_argument("--no-decode", action="store_true", help="skip the decoder throughput block")
     ap.add_argument("--no-parity", action="store_true", help="skip the reference comparison of the produced bitstreams")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step returned to DIR/*.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     rank = int(os.environ.get("RANK", "0"))
@@ -401,14 +407,16 @@ def main():
         aus = [[] for _ in range(S)] if keep else None
         kern, d2h, coded_mbs = [], [], []
         nb = 0
+        last = None                                                # (access units, frame types) of the last collect
 
         def loop(first, count, timed):
-            nonlocal nb
+            nonlocal nb, last
             enc.submit(srcs(first, on_dev, **kw), on_device=on_dev)
             for i in range(1, count + 1):
                 if i < count:
                     enc.submit(srcs(first + i, on_dev, **kw), on_device=on_dev)
-                bs, _ = enc.collect()
+                bs, ft = enc.collect()
+                last = (bs, ft)
                 if keep:
                     for s in range(S):
                         aus[s].append(bs[s])
@@ -437,7 +445,7 @@ def main():
         sampler.join(timeout=2)
         dt, pics = shard.job_totals(max(wall, dev), S * steps, device="cuda")   # MAX over ranks / SUM over ranks
         return {"dt": dt, "pictures": pics, "wall": wall, "dev": dev, "bytes": nb, "clocks": sampler.summary(), "kern": kern, "d2h": d2h,
-                "coded": coded_mbs, "aus": aus}
+                "coded": coded_mbs, "aus": aus, "last": last}
 
     results = {}
     launches0 = L.b2h264_launch_count()
@@ -448,6 +456,8 @@ def main():
         results[mode] = timed_run(enc, mode == "resident", args.warmup, args.steps, keep)
         enc.close()
     launches = L.b2h264_launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *results["resident"]["last"])
 
     # ---- the same workload through the reference's API (ISVCEncoder objects behind the batching broker) ----
     api = None
@@ -548,7 +558,6 @@ def main():
             "clocks": res["clocks"],
             "roofline": {"bound": "hbm", "kernel": "k_encode_mbs (macroblock wavefront, all streams)", "achieved": achieved, "peak": peak,
                          "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": (ncu_traffic("k_encode_mbs") or {}).get("dram_bytes") if S == (ncu_traffic("k_encode_mbs") or {}).get("streams") else None,
                          "peak_source": peak_kind,
                          "note": "wavefront kernel is dependency/latency-bound by construction (SURVEY.md §8d); "
                                  "alg bytes = %d B/MB x %d MB/launch" % (ALG_BYTES_PER_MB, S * MBS_PER_FRAME)},

@@ -2,7 +2,7 @@
  * include/b2h264_codec.h — C-ABI of libopenh264_b200.so, layers 2 and 3: frame-level encoding.
  *
  * Layer 2 — batched frame encoder (b2h264_enc_*): N independent streams of identical geometry are coded
- * together, one picture per stream per call.  This is the B200-shaped entry point: the macroblock loop
+ * together, one picture per stream per call.  This is the GPU-shaped entry point: the macroblock loop
  * of the reference (WelsCodeOneSlice -> WelsISliceMdEnc / WelsMdInterMbLoop,
  * codec/encoder/core/src/svc_encode_slice.cpp:534,1642,1807) plus PerformDeblockingFilter
  * (deblocking.cpp:744) and ExpandReferencingPicture (expand_pic.cpp:388) run on the GPU as a wavefront

@@ -119,7 +119,7 @@ _inited = False
 
 
 def build(verbose=False):
-    """Compile libopenh264_b200.so in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile libopenh264_b200.so in-tree for sm_90a (H100) (nvcc cross-compiles without a GPU)."""
     subprocess.check_call(["make", "-C", os.path.join(HERE, "csrc"), "-j", "8"] + ([] if verbose else ["-s"]))
 
 

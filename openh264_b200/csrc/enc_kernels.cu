@@ -1,4 +1,4 @@
-// enc_kernels.cu — frame-level CUDA kernels of the encoder path (sm_100a):
+// enc_kernels.cu — frame-level CUDA kernels of the encoder path (sm_90a):
 //   k_pad_source     source I420 -> MB-aligned current picture
 //   k_encode_mbs     macroblock mode decision + coding + reconstruction, ONE WARP PER MACROBLOCK; the MBs of
 //                    all streams of the batch are scheduled by dependency (ready list, persistent warps)
@@ -87,7 +87,7 @@ __global__ void __launch_bounds__(256) k_vaa_sad8x8(const StreamFrame* __restric
 // top and top-left neighbours.  Every finished MB notifies its right neighbour and its bottom-left
 // neighbour; the second notification pushes the MB onto a global ready list.  Persistent warps pop the
 // list: no warp ever holds an SM slot while a row it depends on is still busy (a row-per-warp wavefront
-// spent >80% of its issue slots spinning, profiles/r01_encode_rows_ncu.txt).
+// spent most of its issue slots spinning).
 struct Sched {
   int* dep;        // per (stream, mb): notifications received so far
   int* queue;      // ready list, capacity = n_streams * n_mb, -1 = not yet pushed
@@ -135,7 +135,7 @@ __device__ __forceinline__ void run_mbs(const StreamFrame* sf, int n_streams, co
 
 // ---- staged lock-step scheduler of the encode kernel -------------------------------------------------------------
 // The SM's instruction cache holds ~32 KB; the code one macroblock walks through is several times that.  Warps
-// that execute different code thrash it (profiles/r01_encode_icache.txt), warps that start the same code together
+// that execute different code thrash it, warps that start the same code together
 // share every fill.  So (1) the CTA claims up to ENC_WPC tasks AT ONCE, its warps start them together and meet
 // again before the next batch, and (2) a batch is homogeneous: a macroblock is coded in stages (enc_inter.cuh:
 // A skip test, B motion search + inter coding, C intra branch; I = a whole IDR-picture macroblock), every stage has
@@ -152,7 +152,7 @@ struct EncSched {
                      // runs beside this one follows it
 };
 // The control words are spread over NQ + 1 lines (different L2 slices): every finished macroblock, every push and every
-// scheduler look / claim of 148 CTAs used to hit ONE line, and the queueing there slowed the workers' own atomics.
+// scheduler look / claim of one CTA per SM used to hit ONE line, and the queueing there slowed the workers' own atomics.
 __device__ __forceinline__ int* ctl_head(const EncSched& q, int k) { return q.ctl + 32 * k; }
 __device__ __forceinline__ int* ctl_tail(const EncSched& q, int k) { return q.ctl + 32 * k + 1; }
 __device__ __forceinline__ int* ctl_done(const EncSched& q) { return q.ctl + 32 * NQ; }
@@ -248,8 +248,7 @@ __device__ __forceinline__ void run_task(const StreamFrame* sf, const EncSched& 
 // only claims ahead when that cannot starve anybody: a FULL batch once the first worker has finished (or at any time when
 // the list holds two batches' worth); a partial batch only when the workers are already waiting — exactly the decision
 // thread 0 used to take at that moment.  (Experiments that gave up the common start of a batch — warp-asynchronous
-// draws, 2 x 12 and 3 x 8 warp groups — lost 1.4-2.9x to instruction-cache misses: profiles/r01_encode_icache.txt,
-// profiles/r02_encode_variants.txt.)
+// draws, 2 x 12 and 3 x 8 warp groups — lost more than they saved to instruction-cache misses.)
 struct BatchSlot { int k, base, n, pad; };
 constexpr int kEncThreads = 32 * (ENC_WPC + 1);
 __device__ __forceinline__ void enc_cta_barrier() { asm volatile("barrier.sync 1, %0;" ::"n"(kEncThreads) : "memory"); }
@@ -460,10 +459,9 @@ __global__ void __launch_bounds__(kEncThreads, ENC_MIN_CTAS) k_encode_mbs(const 
 // shared memory per SM).  Launched with k_encode_mbs it follows the encode wavefront through `enc_prog` (macroblock (x, y) may be
 // filtered once (x + 1, y + 1) is coded: nothing reads its unfiltered samples any more); both instantiations draw rows from
 // the same counter, so the full-size grid finishes what the resident CTAs have not claimed.  It works (bit-exact, sanitizer
-// clean, steps aside where kernels are serialised) and it does hide the filter — deblock + expand 8.0 -> 4.4 ms per 256 pictures —
-// but the encode kernel beside it takes 73.2 ms instead of 50.7: a fifth instruction stream on every SM evicts the lock-step
-// batch's code from the instruction caches, the same effect as splitting the batch (profiles/r02_encode_variants.txt).
-// Net 78.8 against 59.5 ms per step (gpurun_out/rv -> profiles/r02_bench_lines.txt): off by default.
+// clean, steps aside where kernels are serialised) and it does hide the filter, but the encode
+// kernel beside it slows down by more: a fifth instruction stream on every SM evicts the lock-step batch's code from the
+// instruction caches, the same effect as splitting the batch.  Slower per step overall: off by default.
 #define DBK_WPC 8
 #define DBK_CO_WPC 4
 template <int WPC, int MIN_CTAS, bool BSL = false /* decoder: the pictures may hold B macroblocks (two reference lists in the strength rule) */>

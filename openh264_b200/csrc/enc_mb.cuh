@@ -79,7 +79,7 @@ struct alignas(128) MbScratch {
   int16_t dc16[16];
   int32_t red[32];              // small scratch
   // kept in the scratch rather than on the per-thread stack: the stack of 768 threads does not fit L1 next to the
-  // scratches, and these are touched all the time (profiles/r01_encode_stages.txt)
+  // scratches, and these are touched all the time
   MbCtx ctx;                    // frame parameters / pointers / position of the macroblock being coded
   MeState me[9];                // 16x16, 16x8 x2, 8x16 x2, 8x8 x4 (warp-uniform; written by lane 0)
   int16_t mvcand[5][2];         // 16x16 search candidates
@@ -200,8 +200,7 @@ MBK_HD void mb_load_borders(const MbCtx& c, MbScratch& s) {
 
 // Fused form of mb_load_neighbors + mb_load_cur + mb_load_borders: every lane first ISSUES all of its loads
 // (11 independent global loads in flight: neighbour records, SAD history, current MB, border samples) and only
-// then stores to the scratch, so the macroblock pays one memory latency here instead of five serialized ones
-// (profiles/r01_phase_cycles.txt: 12k cycles/MB before).
+// then stores to the scratch, so the macroblock pays one memory latency here instead of five serialized ones.
 MBK_STAGE void mb_load_all(const MbCtx& c, MbScratch& s) {
   const int mbw = c.p.mb_w, idx = c.mby * mbw + c.mbx, l = lane_id();
   constexpr int kW = (int)(sizeof(MbInfo) / 4);

@@ -455,11 +455,11 @@ __device__ __forceinline__ uint2 qpel8(uint32_t p, int P, int fx, int fy) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// TMA form of the tiled unit (sm_100a: cp.async.bulk.tensor + mbarrier complete_tx).  Same tile geometry; ONE
+// TMA form of the tiled unit (sm_90a: cp.async.bulk.tensor + mbarrier complete_tx).  Same tile geometry; ONE
 // thread issues two bulk tensor copies (current tile 128 x 64, reference tile + halo 160 x 85) and every warp
 // waits on the mbarrier: no per-thread address arithmetic for staging, out-of-picture parts are zero-filled by
-// the copy engine.  ncu on the cp.async form showed the SMs issue-bound (89 % issue-active, 187 warp instructions
-// per macroblock, a third of them staging arithmetic): profiles/r01_mc_sad_ncu.txt.
+// the copy engine.  The cp.async form left the SMs issue-bound, with about a third of the
+// warp instructions per macroblock spent on staging arithmetic.
 // 6 CTAs per SM (40 registers): the packed interpolation needs them; the integer path loses nothing measurable against 8
 __global__ void __launch_bounds__(32 * MCT_W, 6)
 k_mc_sad_tma(const __grid_constant__ CUtensorMap tm_cur, const __grid_constant__ CUtensorMap tm_ref, int mb_w, int mb_h,

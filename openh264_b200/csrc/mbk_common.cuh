@@ -1,4 +1,4 @@
-// mbk_common.cuh — shared device helpers for the macroblock kernels (sm_100a).
+// mbk_common.cuh — shared device helpers for the macroblock kernels (sm_90a).
 //
 // Execution model used throughout: ONE WARP OWNS ONE MACROBLOCK (or one block-level job).
 // Every warp-level routine below must be called by all 32 lanes of a converged warp; results
@@ -16,16 +16,15 @@
 // MBK_WS == 1, so every lane-strided loop visits all indices and warp reductions are the identity.
 #define MBK_HD __host__ __device__ __forceinline__
 // Warp-level routines are real functions, not inlined: one inlined copy per call site grew the encode
-// kernel to 774 KB of SASS and the warps (each in a different phase of a different macroblock) spent
-// 58% of their cycles waiting for instruction fetch (profiles/r01_encode_icache.txt).
+// kernel several-fold and the warps (each in a different phase of a different macroblock) spent most
+// of their cycles waiting for instruction fetch.
 // External (weak, ODR-merged) linkage on purpose: with `static`, ptxas specialises the calling convention of each
 // function inside the translation unit, and one such specialisation returned a stale register for a field the
-// callee had just stored through a pointer into the caller's frame (me_refine -> MeState::mv_y, r01 debugging
-// notes in profiles/r01_encode_stages.txt).  Externally visible functions follow the standard ABI.  Every
+// callee had just stored through a pointer into the caller's frame (me_refine -> MeState::mv_y).  Externally visible functions follow the standard ABI.  Every
 // translation unit is compiled with the same register cap because nvlink keeps one copy of each function.
 #define MBK_FN inline __host__ __device__ __noinline__
 // stage entry points have ONE call site each: inlined there, they cost no code and save the callee-saved register
-// spill / reload of a real call (17-27 STL + LDL per call: 4 % of the encode kernel's instructions, profiles/r02_encode_local.txt)
+// spill / reload of a real call (a few dozen STL + LDL per call)
 #ifdef B2H264_STAGE_CALLS                  // profiling variant: stage entry points as real calls
 #define MBK_STAGE MBK_FN
 #else

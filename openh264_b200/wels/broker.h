@@ -1,7 +1,7 @@
 // broker.h — process-wide batching broker behind layer 3 (include/b2h264_wels_api.h).
 //
 // The reference's ISVCEncoder is one object per stream and EncodeFrame is synchronous
-// (codec/encoder/plus/src/welsEncoderExt.cpp:375).  The B200 pipeline earns its throughput by coding MANY streams
+// (codec/encoder/plus/src/welsEncoderExt.cpp:375).  The GPU pipeline earns its throughput by coding MANY streams
 // per kernel launch (include/b2h264_codec.h, layer 2).  The broker reconciles the two: ISVCEncoder objects with
 // equal configuration register as streams (slots) of ONE shared b2h264_enc ("pool"); EncodeFrame stages its picture,
 // and the callers that arrive within a short window are coded as one batch — the caller that completes the set

@@ -16,6 +16,39 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ORACLE_SO = os.path.join(ROOT, "oracle", "liboracle.so")
 REFSHIM_SO = os.path.join(ROOT, "oracle", "_ref", "librefshim.so")
 REF_DIR = os.path.join(ROOT, "oracle", "_ref")
+GOLDEN = os.path.join(ROOT, "tests", "golden")
+REF_SRC = os.environ.get("OPENH264_REF", "/root/reference")        # the reference's sources, where they exist (as in build())
+
+
+def reference_vector(rel):
+    """path of a bitstream of the reference's res/ directory (`rel` = "res/<name>"): the committed copy under tests/golden
+    where there is one, else the reference's own file where its sources exist, else None (the vectors of several MB)"""
+    name = os.path.basename(rel)
+    for d in ("conformance", "conformance_b", "rejected"):
+        p = os.path.join(GOLDEN, d, name)
+        if os.path.exists(p):
+            return p
+    p = os.path.join(REF_SRC, rel)
+    return p if os.path.exists(p) else None
+
+
+def reference_clip(name, w, h, n):
+    """the first n pictures of one of the reference's res/*.yuv clips: committed under tests/golden (whole, or the first pictures
+    gzip-compressed under tests/golden/clips), else read from the reference's sources where they exist, else None"""
+    import gzip
+    size = n * w * h * 3 // 2
+    whole = os.path.join(GOLDEN, name)
+    if os.path.exists(whole):
+        data = open(whole, "rb").read()
+    else:
+        pre = [f for f in os.listdir(os.path.join(GOLDEN, "clips")) if f.startswith(name + ".first")]
+        if pre:
+            data = gzip.open(os.path.join(GOLDEN, "clips", pre[0])).read()
+        elif os.path.exists(os.path.join(REF_SRC, "res", name)):
+            data = open(os.path.join(REF_SRC, "res", name), "rb").read(size)
+        else:
+            return None
+    return np.frombuffer(data[:size], np.uint8).copy() if len(data) >= size else None
 
 BLK_DIMS = [(16, 16), (16, 8), (8, 16), (8, 8), (4, 4), (8, 4), (4, 8)]
 

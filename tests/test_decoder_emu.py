@@ -64,27 +64,23 @@ def test_host_decoder_matches_reference_decoder(emu, case):
 
 
 def test_host_decoder_on_the_references_own_clip(emu):
-    clip = "/root/reference/res/CiscoVT2people_320x192_12fps.yuv"
-    if not (h264lib.have_ref() and os.path.exists(clip)):
-        pytest.skip("reference build / clip not on this machine")
-    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-    from make_encoder_golden import ref_encode
-    yuv = np.fromfile(clip, dtype=np.uint8)
-    bs = bytes(ref_encode(yuv, 320, 192, 9, 28, 12.0)[0])
-    nr, rw, rh, want = ref_decode(bs)
-    a = np.frombuffer(bs, np.uint8)
-    out = np.zeros(want.size + 64, np.uint8)
+    """the reference encoder's stream of its own 320x192 clip (tests/golden/make_reference_clip_golden.py) must decode to what
+    the reference decoder made of it"""
+    import hashlib
+    import json
+    name = "ref_CiscoVT2people_320x192_qp28.264"
+    gold = json.load(open(os.path.join(ROOT, "tests", "golden", "reference_clips.json")))["decoder"][name]
+    a = np.fromfile(os.path.join(ROOT, "tests", "golden", name), dtype=np.uint8)
+    out = np.zeros(gold["pictures"] * 320 * 192 * 3 // 2 + 64, np.uint8)
     W, H = C.c_int(), C.c_int()
-    assert emu.emu_decode(a.ctypes.data, len(a), out.ctypes.data, out.size, C.byref(W), C.byref(H)) == nr == 9
-    assert np.array_equal(out[:want.size], want)
+    assert emu.emu_decode(a.ctypes.data, len(a), out.ctypes.data, out.size, C.byref(W), C.byref(H)) == gold["pictures"] == 9
+    assert (W.value, H.value) == (gold["width"], gold["height"])
+    assert hashlib.sha1(out[:out.size - 64].tobytes()).hexdigest() == gold["sha1"]
 
 
 def test_unsupported_streams_are_rejected_not_guessed(emu):
     """a stream with scaling lists (outside the supported class) must come back as a parse error, never as pictures"""
-    path = "/root/reference/res/test_scalinglist_jm.264"
-    if not os.path.exists(path):
-        pytest.skip("reference bitstreams not on this machine")
-    a = np.fromfile(path, dtype=np.uint8)
+    a = np.fromfile(os.path.join(ROOT, "tests", "golden", "rejected", "test_scalinglist_jm.264"), dtype=np.uint8)
     out = np.zeros(1 << 20, np.uint8)
     W, H = C.c_int(), C.c_int()
     assert emu.emu_decode(a.ctypes.data, len(a), out.ctypes.data, out.size, C.byref(W), C.byref(H)) < 0
@@ -92,16 +88,20 @@ def test_unsupported_streams_are_rejected_not_guessed(emu):
 
 def test_reference_conformance_table_exact_or_rejected(emu):
     """every bitstream of the reference's decoder golden table (test/api/decoder_test.cpp) either decodes to the
-    PUBLISHED hash or is rejected as outside the supported stream class — never a wrong picture"""
+    PUBLISHED hash or is rejected as outside the supported stream class — never a wrong picture.  The 31 vectors committed under
+    tests/golden (two of them rejected ones) run everywhere; the 20 larger ones (52 MB) where the reference's sources
+    are, and the claims about them are checked where they ran"""
     import hashlib
     import json
     tab = json.load(open(os.path.join(ROOT, "tests", "golden", "reference_decoder_hashes.json")))["pairs"]
-    if not os.path.exists("/root/reference/" + tab[0][0]):
-        pytest.skip("reference bitstreams not on this machine")
     out = np.zeros(400 << 20, np.uint8)
-    exact, wrong = [], []
+    exact, wrong, ran = [], [], set()
     for path, sha in tab:
-        a = np.fromfile("/root/reference/" + path, dtype=np.uint8)
+        src = h264lib.reference_vector(path)
+        if src is None:
+            continue
+        ran.add(os.path.basename(path))
+        a = np.fromfile(src, dtype=np.uint8)
         W, H = C.c_int(), C.c_int()
         n = emu.emu_decode(a.ctypes.data, len(a), out.ctypes.data, out.size, C.byref(W), C.byref(H))
         if n < 0:
@@ -109,18 +109,21 @@ def test_reference_conformance_table_exact_or_rejected(emu):
         h = hashlib.sha1(out[:n * W.value * H.value * 3 // 2].tobytes()).hexdigest()
         (exact if h == sha else wrong).append(os.path.basename(path))
     assert not wrong, wrong
-    assert {"BA1_Sony_D.jsv", "NL1_Sony_D.jsv", "SVA_BA1_B.264", "SVA_NL1_B.264"} <= set(exact)
+    assert len(ran) >= 31                        # the committed vectors
+    def expect(names):
+        assert set(names) & ran <= set(exact), set(names) & ran - set(exact)
+    expect({"BA1_Sony_D.jsv", "NL1_Sony_D.jsv", "SVA_BA1_B.264", "SVA_NL1_B.264"})
     # CABAC (I and P slices, several slices per picture, I_PCM under CABAC) and the CAVLC I_PCM / multi-reference streams
-    assert {"test_qcif_cabac.264", "test_cif_P_CABAC_slice.264", "test_cif_I_CABAC_slice.264", "test_cif_I_CABAC_PCM.264",
-            "CVPCMNL1_SVA_C.264", "MR2_TANDBERG_E.264"} <= set(exact)
+    expect({"test_qcif_cabac.264", "test_cif_P_CABAC_slice.264", "test_cif_I_CABAC_slice.264", "test_cif_I_CABAC_PCM.264",
+            "CVPCMNL1_SVA_C.264", "MR2_TANDBERG_E.264"})
     # B slices (spatial direct, one or two lists per partition, B_8x8, B_Skip; pictures that leave in POC order), CAVLC and CABAC
-    assert {"Cisco_Men_whisper_640x320_CABAC_Bframe_9.264", "Cisco_Men_whisper_640x320_CAVLC_Bframe_9.264",
-            "Cisco_Adobe_PDF_sample_a_1024x768_CAVLC_Bframe_9.264"} <= set(exact)
+    expect({"Cisco_Men_whisper_640x320_CABAC_Bframe_9.264", "Cisco_Men_whisper_640x320_CAVLC_Bframe_9.264",
+            "Cisco_Adobe_PDF_sample_a_1024x768_CAVLC_Bframe_9.264"})
     # High profile as x264 writes it: 8x8 transform + Intra_8x8, explicit weighted P prediction, chroma QP offset, B pyramids, temporal
     # direct prediction, implicit weights — BASELINE.json configs[3]'s 1080p CABAC stream among them
-    assert {"VID_1920x1080_cabac_temporal_direct.264", "VID_1920x1080_cavlc_temporal_direct.264", "VID_1280x720_cabac_temporal_direct.264",
-            "VID_1280x720_cavlc_temporal_direct.264", "VID_1280x544_cabac_temporal_direct.264", "VID_1280x544_cavlc_temporal_direct.264"} <= set(exact)
-    assert len(exact) >= 49                      # of 51; rejected: scaling lists, SVC subset SPS
+    expect({"VID_1920x1080_cabac_temporal_direct.264", "VID_1920x1080_cavlc_temporal_direct.264", "VID_1280x720_cabac_temporal_direct.264",
+            "VID_1280x720_cavlc_temporal_direct.264", "VID_1280x544_cabac_temporal_direct.264", "VID_1280x544_cavlc_temporal_direct.264"})
+    assert len(ran) - len(exact) <= 2            # of 51; rejected: scaling lists, SVC subset SPS
 
 
 @pytest.mark.parametrize("entropy", [(0, 66), (1, 0)])

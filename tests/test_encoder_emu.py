@@ -1,8 +1,8 @@
 """CPU-side check of the encoder's macroblock pipeline SOURCE: the host emulation build (tests/emu, the same
 enc_*.cuh code compiled as a 1-lane warp and run in raster order) must reproduce the reference encoder's
-bitstream bit for bit — against the golden SHA-1s generated from the reference (tests/golden/encoder.json) and,
-where oracle/_ref exists, against the reference run side by side (incl. the reference's own
-res/CiscoVT2people_320x192_12fps.yuv clip, BASELINE.json config 2).  The GPU build of the same source is
+bitstream bit for bit — against the golden SHA-1s generated from the reference (tests/golden/encoder.json,
+reference_clips.json: incl. the reference's own res/CiscoVT2people_320x192_12fps.yuv clip, BASELINE.json config 2) and,
+where oracle/_ref exists, against the reference run side by side.  The GPU build of the same source is
 checked by tests/test_gpu_encoder.py."""
 import ctypes as C
 import hashlib
@@ -17,6 +17,21 @@ import h264lib
 
 ROOT = h264lib.ROOT
 GOLD = json.load(open(os.path.join(ROOT, "tests", "golden", "encoder.json")))
+# the reference encoder's output on its own res/ clips (tests/golden/make_reference_clip_golden.py)
+CLIPS = json.load(open(os.path.join(ROOT, "tests", "golden", "reference_clips.json")))["encoder"]
+
+
+def check_reference_clip(emu, name, w, h, n, qp, fps, entropy=(0, 66)):
+    """encode the first n pictures of a reference clip in the host build and compare with the reference's stored output;
+    False when the clip is not available (only the 1280x720 clip, which is too large to commit, can be missing)"""
+    g = CLIPS["%s_n%d_qp%d_fps%g_entropy%d_profile%d" % (name, n, qp, fps, entropy[0], entropy[1])]
+    yuv = h264lib.reference_clip(name, w, h, n)
+    if yuv is None:
+        return False
+    assert hashlib.sha1(yuv.tobytes()).hexdigest() == g["clip_sha1"], name
+    bs, fb = emu_encode(emu, yuv, w, h, n, qp, fps, entropy=entropy)
+    assert fb == g["frame_bytes"] and hashlib.sha1(bs).hexdigest() == g["sha1"], (name, qp, entropy)
+    return True
 
 
 @pytest.fixture(scope="module")
@@ -52,17 +67,8 @@ def test_emu_matches_golden(emu, key):
 
 
 def test_emu_matches_reference_on_its_own_clip(emu):
-    clip = "/root/reference/res/CiscoVT2people_320x192_12fps.yuv"
-    if not (h264lib.have_ref() and os.path.exists(clip)):
-        pytest.skip("reference build / clip not on this machine")
-    import sys
-    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-    from make_encoder_golden import ref_encode
-    yuv = np.fromfile(clip, dtype=np.uint8)
     for qp in (26, 34):
-        ref_bs, ref_fb, _ = ref_encode(yuv, 320, 192, 9, qp, 12.0)
-        bs, fb = emu_encode(emu, yuv, 320, 192, 9, qp, 12.0)
-        assert fb == ref_fb and bs == ref_bs
+        assert check_reference_clip(emu, "CiscoVT2people_320x192_12fps.yuv", 320, 192, 9, qp, 12.0)
 
 
 EDGE_CASES = [
@@ -91,29 +97,11 @@ def test_emu_matches_reference_edge_cases(emu, case):
 
 
 def test_emu_matches_reference_on_other_reference_clips(emu):
-    """more of the reference's own res/*.yuv clips (first pictures), where they exist"""
-    if not h264lib.have_ref():
-        pytest.skip("reference build not on this machine")
-    import sys
-    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-    from make_encoder_golden import ref_encode
-    clips = [("/root/reference/res/Cisco_Absolute_Power_1280x720_30fps.yuv", 1280, 720, 2, 30),
-             ("/root/reference/res/CiscoVT2people_160x96_6fps.yuv", 160, 96, 6, 24),
-             ("/root/reference/res/Static_152_100.yuv", 152, 100, 8, 28)]
-    ran = 0
-    for path, w, h, n, qp in clips:
-        if not os.path.exists(path):
-            continue
-        fsz = w * h * 3 // 2
-        yuv = np.fromfile(path, dtype=np.uint8, count=n * fsz)
-        if yuv.size < n * fsz:
-            continue
-        ref_bs, ref_fb, _ = ref_encode(yuv, w, h, n, qp, 30.0)
-        bs, fb = emu_encode(emu, yuv, w, h, n, qp, 30.0)
-        assert fb == ref_fb and bs == bytes(ref_bs), path
-        ran += 1
-    if not ran:
-        pytest.skip("no reference clips on this machine")
+    """more of the reference's own res/*.yuv clips (first pictures); the 1280x720 one only where the reference's sources are"""
+    ran = [check_reference_clip(emu, *c) for c in [("Cisco_Absolute_Power_1280x720_30fps.yuv", 1280, 720, 2, 30, 30.0),
+                                                   ("CiscoVT2people_160x96_6fps.yuv", 160, 96, 5, 24, 30.0),
+                                                   ("Static_152_100.yuv", 152, 100, 8, 28, 30.0)]]
+    assert all(ran[1:])
 
 
 EDGE = json.load(open(os.path.join(ROOT, "tests", "golden", "encoder_edge.json")))
@@ -156,26 +144,10 @@ def test_emu_cabac_matches_reference_golden(emu, key):
 
 
 def test_emu_cabac_matches_reference_side_by_side(emu):
-    """the same, against the compiled reference on its own clips, both profiles"""
-    if not h264lib.have_ref():
-        pytest.skip("reference build not on this machine")
-    import sys
-    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-    from make_encoder_golden import ref_encode
-    clips = [("/root/reference/res/CiscoVT2people_160x96_6fps.yuv", 160, 96, 5, 24), ("/root/reference/res/Static_152_100.yuv", 152, 100, 8, 28)]
-    ran = 0
-    for path, w, h, n, qp in clips:
-        fsz = w * h * 3 // 2
-        if not os.path.exists(path) or os.path.getsize(path) < n * fsz:
-            continue
-        yuv = np.fromfile(path, dtype=np.uint8, count=n * fsz)
+    """the same, against the reference's output on its own clips, both profiles"""
+    for name, w, h, n, qp in [("CiscoVT2people_160x96_6fps.yuv", 160, 96, 5, 24), ("Static_152_100.yuv", 152, 100, 8, 28)]:
         for prof in (0, 77):
-            ref_bs, ref_fb, _ = ref_encode(yuv, w, h, n, qp, 30.0, entropy=(1, prof))
-            bs, fb = emu_encode(emu, yuv, w, h, n, qp, 30.0, entropy=(1, prof))
-            assert fb == ref_fb and bs == bytes(ref_bs), (path, prof)
-        ran += 1
-    if not ran:
-        pytest.skip("no reference clips on this machine")
+            assert check_reference_clip(emu, name, w, h, n, qp, 30.0, entropy=(1, prof))
 
 
 @pytest.mark.parametrize("key", sorted(EDGE["intra_period"]))

@@ -1,5 +1,5 @@
 """Summarise an .ncu-rep (one kernel) as text: duration, throughput, stall mix, memory traffic.
-usage: python tools/ncu_summary.py report.ncu-rep > profiles/xxx.txt"""
+usage: python tools/ncu_summary.py report.ncu-rep > summary.txt"""
 import csv, io, subprocess, sys
 
 rep = sys.argv[1]

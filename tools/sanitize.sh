@@ -1,6 +1,6 @@
 #!/bin/bash
 # compute-sanitizer passes over the small encode + decode (tools/sanitize_small.py); logs -> gpurun_out/
-# (copy the clean ones to profiles/).  Run on the GPU box:  gpurun -- bash tools/sanitize.sh
+# Run on a machine with a GPU and compute-sanitizer:  bash tools/sanitize.sh
 mkdir -p gpurun_out
 for tool in memcheck racecheck synccheck; do
   timeout 240 compute-sanitizer --tool $tool --print-limit 20 python tools/sanitize_small.py > gpurun_out/sanitize_$tool.log 2>&1

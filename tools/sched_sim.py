@@ -1,12 +1,11 @@
 """Discrete-event model of the staged lock-step scheduler of k_encode_mbs (openh264_b200/csrc/enc_kernels.cu).
 
-Why: on the GPU the kernel is bound by its dependency structure (55 % of warp time waits at batch barriers,
-profiles/r01_encode_stages.txt), and scheduler variants cost GPU time to try.  This model replays the REAL
+Why: on the GPU the kernel is bound by its dependency structure (much of the warp time waits at batch barriers), and scheduler variants cost GPU time to try.  This model replays the REAL
 per-macroblock stage paths of the bench clip (recorded by the host build of the macroblock code,
 tools/sim_data/mb_stage_paths_1080p.npy: bit s set = stage s ran; A=1, I=2, Bs=3, B=4, C=5) through the same
-policy — 148 CTAs, W warps each, a batch = up to W ready tasks of ONE stage, batch time = slowest task + a fixed
-overhead, later stages first, a full batch beats a partial one — with the stage costs measured on the B200
-(tools/enc_stats.py).  It is calibrated against the measured kernel times and then used to rank ideas.
+policy — one CTA per SM (132 on an H100), W warps each, a batch = up to W ready tasks of ONE stage, batch time = slowest task + a fixed
+overhead, later stages first, a full batch beats a partial one — with the recorded stage costs
+(tools/enc_stats.py).  The default costs below were not measured on the H100: remeasure them there before ranking ideas.
 
 usage: python tools/sched_sim.py [--streams 256] [--warps 24] [--variant base|dfill|dfull|half|patience|fastB]
 """
@@ -19,7 +18,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 A, I, BS, B, C, D = 1, 2, 3, 4, 5, 6
-# measured cycles per task (256 streams, 24 warps/SM, tools/enc_stats.py): stage -> cycles
+# cycles per task, stage -> cycles: placeholders not measured on the H100 (measure with tools/enc_stats.py)
 COST = {A: 45000, BS: 31500, B: 250000, C: 800000, D: 11200, I: 550000}
 BATCH_OVERHEAD = 3000          # claim + two CTA barriers + park/unpark
 MBW, MBH = 120, 68
@@ -31,7 +30,7 @@ def build_paths(n_streams, seed=1):
     return [paths[rng.randrange(len(paths))] for _ in range(n_streams)]
 
 
-def simulate(n_streams=256, warps=24, n_cta=148, variant="base", seed=1, cost=None, verbose=False):
+def simulate(n_streams=256, warps=24, n_cta=132, variant="base", seed=1, cost=None, verbose=False):
     cost = dict(COST if cost is None else cost)
     if variant == "fastB":
         cost[B] = int(cost[B] * 0.7)
