@@ -263,7 +263,7 @@ int b2h264_enc_submit(b2h264_enc* e, const uint8_t* const* src, int src_on_devic
                             e->have_tmap ? e->tmap_pic : nullptr, e->cfg.complexity_low != 0, e->st);
   if (rc) return rc;
   CK(cudaEventRecord(sl.ev1, e->st));
-  rc = enc_launch_deblock_expand(e->d_sf[k], n, mbw, mbh, e->d_tickets, e->st);
+  rc = enc_launch_deblock_expand(e->d_sf[k], n, mbw, mbh, e->st);
   if (rc) return rc;
   CK(cudaEventRecord(sl.ev2, e->st));
   // the macroblock records are final once the encode kernel is done (deblocking does not touch them)

@@ -2,7 +2,7 @@
 //   k_pad_source     source I420 -> MB-aligned current picture
 //   k_encode_mbs     macroblock mode decision + coding + reconstruction, ONE WARP PER MACROBLOCK; the MBs of
 //                    all streams of the batch are scheduled by dependency (ready lists, persistent warps)
-//   k_deblock_rows   in-loop deblocking, one warp per macroblock row (encoder and decoder)
+//   k_deblock_pictures  in-loop deblocking, one CTA per picture, one warp per macroblock row (encoder and decoder)
 //   k_decode_mbs     the decoder's macroblock reconstruction, scheduled like the encoder's macroblocks
 //   k_expand_*       border replication of the new reference picture (ExpandReferencingPicture)
 // Why a wavefront: MB(x,y) needs the FINAL state of (x-1,y), (x,y-1), (x+1,y-1) — motion-vector / SAD
@@ -435,48 +435,55 @@ __global__ void __launch_bounds__(kEncThreads, 1) k_encode_mbs(const StreamFrame
   });
 }
 
-// In-loop deblocking: ONE WARP PER MACROBLOCK ROW.  The tasks are short and uniform (a few microseconds each), so the
-// dependency bookkeeping of the general scheduler (two global atomics, a fence and a polled ready list per macroblock) cost
-// more than the filtering itself: 9.4 ms per 256 x 1080p pictures, 1900 warp instructions per macroblock.  Here a warp walks
-// its row left to right and only has to stay two macroblocks behind the row above (MB(x, y) needs (x - 1, y) — the warp's own
-// previous step — and (x + 1, y - 1)); progress is one int per row.  Rows are handed out row-major over the streams (all
-// rows 0 first), so a row is only ever claimed after the row it waits for: no deadlock whatever the number of resident warps.
-// The grid is full-size (6 CTAs of 8 warps per SM) and launched behind the encode kernel.  (Deblocking CTAs resident beside the
-// encode kernel, following its wavefront, hid the filter but slowed the encode kernel by more: DESIGN.md §7.)
-#define DBK_WPC 8
-template <int WPC, int MIN_CTAS, bool BSL = false /* decoder: the pictures may hold B macroblocks (two reference lists in the strength rule) */>
-__global__ void __launch_bounds__(32 * WPC, MIN_CTAS) k_deblock_rows(const StreamFrame* __restrict__ sf, int n_streams, int* prog, int* counter) {
+// In-loop deblocking: ONE CTA PER PICTURE, ONE WARP PER MACROBLOCK ROW AT A TIME.  The warps of a CTA take the rows of
+// their picture round-robin; a warp walks its row left to right and only has to stay two macroblocks behind the row above
+// (MB(x, y) needs (x - 1, y) — the warp's own previous step — and (x + 1, y - 1)).  Progress is one word per warp in shared
+// memory, ordered with CTA-scope release / acquire: the whole wavefront of a picture lives on one SM, so no GPU-scope fence,
+// no global counter and no L1 invalidation are needed (the round-1 version spread the rows of all pictures over the chip
+// and paid two GPU-scope fences per macroblock; the staged filter waited mostly for its loads).  Per macroblock a warp
+// fetches the next macroblock's own samples and records asynchronously before it filters this one (deblock_row_t), so only
+// the 4 rows above wait on another warp.  Launched behind the encode kernel.  (Deblocking CTAs resident beside the encode
+// kernel, following its wavefront, hid the filter but slowed the encode kernel by more: DESIGN.md §7.)
+#define DBK_MAX_WARPS 32
+#define DBK_WARPS_SHARED 17       // two CTAs per SM: 68-row (1080p) pictures give every warp 4 rows
+__device__ __forceinline__ int ld_acquire_cta(const int* p) {
+  int v;
+  asm volatile("ld.acquire.cta.shared.b32 %0, [%1];" : "=r"(v) : "r"((unsigned)__cvta_generic_to_shared(p)) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_cta(int* p, int v) {
+  asm volatile("st.release.cta.shared.b32 [%0], %1;" ::"r"((unsigned)__cvta_generic_to_shared(p)), "r"(v) : "memory");
+}
+// __maxnreg__(56): two CTAs of DBK_WARPS_SHARED warps fit the register file (60 registers, the uncapped count, allow one)
+template <bool BSL = false /* decoder: the pictures may hold B macroblocks (two reference lists in the strength rule) */>
+__global__ void __maxnreg__(56) k_deblock_pictures(const StreamFrame* __restrict__ sf) {
   using Tile = typename std::conditional<BSL, DbkTileB, DbkTile>::type;
-  __shared__ Tile tiles[WPC];
-  Tile& t = tiles[threadIdx.x >> 5];
-  const int lane = threadIdx.x & 31;
-  const int mb_w = sf[0].p.mb_w, mb_h = sf[0].p.mb_h, units = n_streams * mb_h;
-  for (;;) {
-    int u = 0;
-    if (lane == 0) u = atomicAdd(counter, 1);
-    u = __shfl_sync(MBK_FULL, u, 0);
-    if (u >= units) break;
-    const int row = u / n_streams, si = u - row * n_streams;
-    const StreamFrame& F = sf[si];
-    int* mine = prog + si * mb_h + row;
-    const int* up = mine - 1;
-    int seen = row > 0 ? 0 : mb_w;
-    for (int x = 0; x < mb_w; x++) {
-      const int need = x + 2 < mb_w ? x + 2 : mb_w;
-      if (seen < need) {
-        if (lane == 0) {
-          while ((seen = ld_volatile(up)) < need) __nanosleep(40);
-        }
-        seen = __shfl_sync(MBK_FULL, seen, 0);
-        __threadfence();
-      }
-      deblock_one_mb_t<BSL>(F.p, F.f, x, row, t);
-      __threadfence();
-      __syncwarp();
-      if (lane == 0) *reinterpret_cast<volatile int*>(mine) = x + 1;
-    }
+  extern __shared__ __align__(16) uint8_t dbk_smem[];
+  __shared__ int s_done[DBK_MAX_WARPS];                    // macroblocks finished by each warp, counted as row * mb_w + x + 1
+  const int nw = blockDim.x >> 5, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const StreamFrame& F = sf[blockIdx.x];
+  const int mb_w = F.p.mb_w, mb_h = F.p.mb_h;
+  Tile* t = reinterpret_cast<Tile*>(dbk_smem) + 2 * w;
+  if (threadIdx.x < DBK_MAX_WARPS) s_done[threadIdx.x] = 0;
+  __syncthreads();
+  const int* above = &s_done[w > 0 ? w - 1 : nw - 1];
+  int* mine = &s_done[w];
+  for (int row = w; row < mb_h; row += nw) {
+    const int base = (row - 1) * mb_w;
+    deblock_row_t<BSL>(F.p, F.f, row, t,
+        [&](int need) {
+          if (lane == 0)
+            while (ld_acquire_cta(above) < base + need) __nanosleep(32);
+          __syncwarp();
+        },
+        [&](int x) {
+          __syncwarp();
+          if (lane == 0) st_release_cta(mine, base + mb_w + x + 1);
+        });
   }
 }
+template <bool BSL>
+static size_t dbk_tile_bytes() { return sizeof(typename std::conditional<BSL, DbkTileB, DbkTile>::type); }
 
 // ---- decoder construct path (groundwork of the next SURVEY row: dec_mb.cuh) ------------------------------------------------
 // One warp reconstructs one macroblock from its parsed record (h264_parse.h); the macroblocks of all streams are
@@ -570,20 +577,17 @@ static int dec_grid_blocks() {
 }
 
 // ---- scheduler workspace (ints), one layout for the encoder (NQ ready lists) and the decoder (one list) ------------------
-//   [0]                       row hand-out counter of k_deblock_rows
-//   prog[n_streams * mb_h]    k_deblock_rows: macroblocks deblocked per row
 //   dep[total]                notifications received per macroblock (total = n_streams * n_mb)
 //   queue[n_lists][total]     ready lists, -1 = slot not yet written
 //   ctl[32 * (n_lists + 1)]   control lines: the encoder's per list (EncSched), the decoder's head and tail (Sched)
 // Every part starts on a 128-byte line.  Per picture [0, queue) is zeroed and the lists are set to -1 (sched_ws_reset); the
 // control lines are written by k_esched_init / k_sched_init.
-struct SchedWs { size_t prog, dep, queue, ctl, ints; };
+struct SchedWs { size_t dep, queue, ctl, ints; };
 static size_t ws_lines(size_t n) { return (n + 31) / 32 * 32; }
 static SchedWs sched_ws(int n_streams, int mb_w, int mb_h, int n_lists) {
   const size_t total = (size_t)n_streams * mb_w * mb_h;
   SchedWs w;
-  w.prog = 32;
-  w.dep = w.prog + ws_lines((size_t)n_streams * mb_h);
+  w.dep = 0;
   w.queue = w.dep + ws_lines(total);
   w.ctl = w.queue + ws_lines((size_t)n_lists * total);
   w.ints = w.ctl + 32 * ((size_t)n_lists + 1);
@@ -605,24 +609,33 @@ static EncSched make_esched(int* ws, const SchedWs& w, void* stash) {
   return q;
 }
 
-// prog: n_streams * mb_h progress counters, zero; counter: the row hand-out counter, zero
-static int launch_deblock_rows(const StreamFrame* d_sf, int n_streams, int mb_h, int* prog, int* counter, cudaStream_t st, bool b_slices = false) {
-  static int per_dev[64];
-  int dev = 0, sms = 0;
+// One CTA per picture.  With enough pictures for two CTAs per SM a CTA has DBK_WARPS_SHARED warps; a small batch (a single
+// encoder or decoder object) has the SMs to itself and gives each picture DBK_MAX_WARPS warps, which shortens the row pipeline
+// of a picture.
+template <bool BSL>
+static int launch_deblock_t(const StreamFrame* d_sf, int n_streams, int mb_h, cudaStream_t st) {
+  static std::mutex mu;
+  static int sms_dev[64];
+  int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64) dev = 0;
-  if (!per_dev[dev]) {
-    int per_sm = 0;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_deblock_rows<DBK_WPC, 6>, 32 * DBK_WPC, 0);
-    per_dev[dev] = sms * (per_sm < 1 ? 1 : per_sm);
+  int sms;
+  {
+    std::lock_guard<std::mutex> lock(mu);
+    if (!sms_dev[dev]) {
+      cudaFuncSetAttribute(k_deblock_pictures<BSL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * DBK_MAX_WARPS * dbk_tile_bytes<BSL>()));
+      cudaDeviceGetAttribute(&sms_dev[dev], cudaDevAttrMultiProcessorCount, dev);
+      if (sms_dev[dev] < 1) sms_dev[dev] = 1;
+    }
+    sms = sms_dev[dev];
   }
-  const int units = n_streams * mb_h;
-  int blocks = per_dev[dev];
-  if (blocks > (units + DBK_WPC - 1) / DBK_WPC) blocks = (units + DBK_WPC - 1) / DBK_WPC;
-  if (b_slices) k_deblock_rows<DBK_WPC, 6, true><<<blocks, 32 * DBK_WPC, 0, st>>>(d_sf, n_streams, prog, counter);
-  else k_deblock_rows<DBK_WPC, 6><<<blocks, 32 * DBK_WPC, 0, st>>>(d_sf, n_streams, prog, counter);
+  int nw = 2 * n_streams > sms ? DBK_WARPS_SHARED : DBK_MAX_WARPS;
+  if (nw > mb_h) nw = mb_h;
+  k_deblock_pictures<BSL><<<n_streams, 32 * nw, 2 * nw * dbk_tile_bytes<BSL>(), st>>>(d_sf);
   return b2h264_launched();
+}
+static int launch_deblock(const StreamFrame* d_sf, int n_streams, int mb_h, cudaStream_t st, bool b_slices = false) {
+  return b_slices ? launch_deblock_t<true>(d_sf, n_streams, mb_h, st) : launch_deblock_t<false>(d_sf, n_streams, mb_h, st);
 }
 
 int enc_launch_frame(const StreamFrame* d_sf, const uint8_t* const* d_src, int n_streams, int w, int h, int mb_w, int mb_h,
@@ -640,7 +653,7 @@ int enc_launch_frame(const StreamFrame* d_sf, const uint8_t* const* d_src, int n
   }
   const int total = n_streams * mb_w * mb_h;
   const SchedWs ws = sched_ws(n_streams, mb_w, mb_h, NQ);
-  sched_ws_reset(d_ws, ws, st);                       // also the deblocking counters enc_launch_deblock_expand uses
+  sched_ws_reset(d_ws, ws, st);
   const EncSched qe = make_esched(d_ws, ws, d_stash);
   k_esched_init<<<1, 32, 0, st>>>(qe, d_sf, n_streams, mb_w * mb_h);
   int blocks = enc_grid_blocks();
@@ -654,10 +667,9 @@ int enc_launch_frame(const StreamFrame* d_sf, const uint8_t* const* d_src, int n
   return b2h264_launched();
 }
 
-int enc_launch_deblock_expand(const StreamFrame* d_sf, int n_streams, int mb_w, int mb_h, int* d_ws, cudaStream_t st) {
+int enc_launch_deblock_expand(const StreamFrame* d_sf, int n_streams, int mb_w, int mb_h, cudaStream_t st) {
   int rc;
-  const SchedWs ws = sched_ws(n_streams, mb_w, mb_h, NQ);       // counter and progress words: zeroed by enc_launch_frame
-  if ((rc = launch_deblock_rows(d_sf, n_streams, mb_h, d_ws + ws.prog, d_ws, st))) return rc;
+  if ((rc = launch_deblock(d_sf, n_streams, mb_h, st))) return rc;
   k_expand_lr_batch<<<dim3((mb_h * 16 + 7) / 8, 1, 3 * n_streams), dim3(32, 8), 0, st>>>(d_sf);
   if ((rc = b2h264_launched())) return rc;
   k_expand_tb_batch<<<dim3((mb_w * 16 + 64 + 127) / 128, 4, 3 * n_streams), dim3(128), 0, st>>>(d_sf);
@@ -684,7 +696,7 @@ int dec_launch_frame(const StreamFrame* d_sf, int n_streams, int mb_w, int mb_h,
   const int need = (total + DEC_WPC - 1) / DEC_WPC;
   k_decode_mbs<<<blocks_per_launch < need ? blocks_per_launch : need, 32 * DEC_WPC, kScratchSmem, st>>>(d_sf, n_streams, qc, d_recs, d_aux);
   if ((rc = b2h264_launched())) return rc;
-  if (deblock && (rc = launch_deblock_rows(d_sf, n_streams, mb_h, d_ws + ws.prog, d_ws, st, b_slices != 0))) return rc;
+  if (deblock && (rc = launch_deblock(d_sf, n_streams, mb_h, st, b_slices != 0))) return rc;
   k_expand_lr_batch<<<dim3((mb_h * 16 + 7) / 8, 1, 3 * n_streams), dim3(32, 8), 0, st>>>(d_sf);
   if ((rc = b2h264_launched())) return rc;
   k_expand_tb_batch<<<dim3((mb_w * 16 + 64 + 127) / 128, 4, 3 * n_streams), dim3(128), 0, st>>>(d_sf);

@@ -17,8 +17,8 @@ int enc_launch_frame(const StreamFrame* d_sf, const uint8_t* const* d_src, int n
                      const void* tmap_ref /* CUtensorMap of the reference luma planes or NULL: the search reads the planes directly */,
                      int fast_mode /* LOW_COMPLEXITY: also computes the VAA 8x8 SADs */, cudaStream_t st);
 // wavefront deblocking + border expansion of the pictures just reconstructed
-int enc_launch_deblock_expand(const StreamFrame* d_sf, int n_streams, int mb_w, int mb_h, int* d_sched_ws, cudaStream_t st);
-// number of ints of scheduler workspace (deblocking counters, dependency counters, ready lists) for a batch
+int enc_launch_deblock_expand(const StreamFrame* d_sf, int n_streams, int mb_w, int mb_h, cudaStream_t st);
+// number of ints of scheduler workspace (dependency counters, ready lists) for a batch
 size_t enc_sched_ints(int n_streams, int mb_w, int mb_h);
 size_t enc_stash_bytes(int n_streams, int mb_h);      // parked macroblock scratches (one per stream and MB row)
 size_t enc_scratch_bytes();
