@@ -10,6 +10,7 @@
 // that chain, so parallelism comes from rows (2-MB lag) x independent streams of the batch.
 #include <cuda.h>
 #include <type_traits>
+#include <vector>
 #include <stddef.h>
 #include <stdlib.h>
 #include <string.h>
@@ -611,9 +612,9 @@ static EncSched make_esched(int* ws, const SchedWs& w, void* stash) {
 
 // One CTA per picture.  With enough pictures for two CTAs per SM a CTA has DBK_WARPS_SHARED warps; a small batch (a single
 // encoder or decoder object) has the SMs to itself and gives each picture DBK_MAX_WARPS warps, which shortens the row pipeline
-// of a picture.
+// of a picture.  n_warps > 0 replaces that choice (still capped at mb_h); *warps_used receives the count launched.
 template <bool BSL>
-static int launch_deblock_t(const StreamFrame* d_sf, int n_streams, int mb_h, cudaStream_t st) {
+static int launch_deblock_t(const StreamFrame* d_sf, int n_streams, int mb_h, cudaStream_t st, int n_warps = 0, int* warps_used = nullptr) {
   static std::mutex mu;
   static int sms_dev[64];
   int dev = 0;
@@ -629,10 +630,55 @@ static int launch_deblock_t(const StreamFrame* d_sf, int n_streams, int mb_h, cu
     }
     sms = sms_dev[dev];
   }
-  int nw = 2 * n_streams > sms ? DBK_WARPS_SHARED : DBK_MAX_WARPS;
+  int nw = n_warps > 0 ? n_warps : 2 * n_streams > sms ? DBK_WARPS_SHARED : DBK_MAX_WARPS;
   if (nw > mb_h) nw = mb_h;
+  if (warps_used) *warps_used = nw;
   k_deblock_pictures<BSL><<<n_streams, 32 * nw, 2 * nw * dbk_tile_bytes<BSL>(), st>>>(d_sf);
   return b2h264_launched();
+}
+
+// Test hook (not part of the public headers): deblocks n pictures given as device planes and records, through the same
+// launcher as the encoder and the decoder.  planes[3 * i + pl] = sample (0, 0) of plane pl of picture i; geo[4 * i] = luma
+// stride, chroma stride, mb_w, mb_h; mbi[i] = its MbInfo records, aux_b[i] = its DecMbAuxB records or NULL (aux_b itself may
+// be NULL).  dec_mode 1 reads the slice control from the records, 0 uses idc / off_a / off_b.  bsl selects the two-list
+// instantiation (required for B records and the 8x8 transform).  n_warps 0 lets the launcher choose.  Returns -1 without
+// launching when an argument does not fit the kernel's accesses (16-byte luma rows, 8-byte chroma rows, 16-byte aligned
+// plane origins); otherwise the CUDA status after the kernel finished, with the warp count in *warps_used.
+extern "C" int b2h264_debug_deblock_pictures(int n, uint8_t* const* planes, const int* geo, MbInfo* const* mbi,
+                                             const DecMbAuxB* const* aux_b, int dec_mode, int idc, int off_a, int off_b, int bsl,
+                                             int n_warps, int* warps_used) {
+  if (n < 1 || !planes || !geo || !mbi || n_warps < 0 || n_warps > DBK_MAX_WARPS) return -1;
+  int max_h = 1;
+  for (int i = 0; i < n; i++) {
+    const int sy = geo[4 * i], sc = geo[4 * i + 1], mb_w = geo[4 * i + 2], mb_h = geo[4 * i + 3];
+    if (mb_w < 1 || mb_h < 1 || sy % 16 || sc % 8 || sy < 16 * mb_w || sc < 8 * mb_w || !mbi[i]) return -1;
+    for (int pl = 0; pl < 3; pl++)
+      if (!planes[3 * i + pl] || reinterpret_cast<uintptr_t>(planes[3 * i + pl]) % 16) return -1;
+    if (aux_b && aux_b[i] && !bsl) return -1;
+    if (mb_h > max_h) max_h = mb_h;
+  }
+  int rc = enc_upload_deblock_tables();            // as b2h264_enc_create / b2h264_dec_create do
+  if (rc) return rc;
+  std::vector<StreamFrame> h(n);
+  memset(h.data(), 0, sizeof(StreamFrame) * n);
+  for (int i = 0; i < n; i++) {
+    EncFrameParams& p = h[i].p;
+    p.rec_stride_y = geo[4 * i]; p.rec_stride_c = geo[4 * i + 1]; p.mb_w = geo[4 * i + 2]; p.mb_h = geo[4 * i + 3];
+    p.dec_mode = dec_mode; p.dbk_idc = idc; p.dbk_off_a = off_a; p.dbk_off_b = off_b;
+    for (int pl = 0; pl < 3; pl++) h[i].f.rec[pl] = planes[3 * i + pl];
+    h[i].f.mbi = mbi[i];
+    h[i].f.dec_aux_b = aux_b ? aux_b[i] : nullptr;
+  }
+  StreamFrame* d_sf = nullptr;
+  cudaError_t e = cudaMalloc(&d_sf, sizeof(StreamFrame) * n);
+  if (e != cudaSuccess) return (int)e;
+  rc = (int)cudaMemcpy(d_sf, h.data(), sizeof(StreamFrame) * n, cudaMemcpyHostToDevice);
+  int used = 0;
+  if (!rc) rc = bsl ? launch_deblock_t<true>(d_sf, n, max_h, 0, n_warps, &used) : launch_deblock_t<false>(d_sf, n, max_h, 0, n_warps, &used);
+  if (!rc) rc = (int)cudaDeviceSynchronize();
+  cudaFree(d_sf);
+  if (warps_used) *warps_used = used;
+  return rc;
 }
 static int launch_deblock(const StreamFrame* d_sf, int n_streams, int mb_h, cudaStream_t st, bool b_slices = false) {
   return b_slices ? launch_deblock_t<true>(d_sf, n_streams, mb_h, st) : launch_deblock_t<false>(d_sf, n_streams, mb_h, st);

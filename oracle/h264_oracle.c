@@ -550,6 +550,147 @@ void orc_deblock_chroma_eq4 (uint8_t* cb, uint8_t* cr, int sx, int sy, int alpha
 }
 
 /* ------------------------------------------------------------------------------------------
+ * Whole-picture deblocking, H.264 8.7, macroblocks in raster order.  Boundary strengths follow
+ * 8.7.2.1 with the departures of the reference decoder (decoder/core/src/deblocking.cpp) marked
+ * where they occur; the edge filters are the ones above.
+ * ------------------------------------------------------------------------------------------ */
+/* Table 8-16: alpha' and beta' by indexA / indexB */
+static const uint8_t kDbkAlpha[52] = {
+  0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 4, 4, 5, 6, 7, 8, 9, 10, 12, 13,
+  15, 17, 20, 22, 25, 28, 32, 36, 40, 45, 50, 56, 63, 71, 80, 90, 101, 113, 127, 144, 162, 182, 203, 226, 255, 255};
+static const uint8_t kDbkBeta[52] = {
+  0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 2, 2, 2, 3, 3, 3, 3, 4, 4, 4,
+  6, 6, 7, 7, 8, 8, 9, 9, 10, 10, 11, 11, 12, 12, 13, 13, 14, 14, 15, 15, 16, 16, 17, 17, 18, 18};
+/* Table 8-17: tC0 by bS (rows 1..3) and indexA */
+static const uint8_t kDbkTc0[3][52] = {
+  {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1,
+   1, 1, 1, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 4, 4, 4, 5, 6, 6, 7, 8, 9, 10, 11, 13},
+  {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 1,
+   1, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 4, 4, 5, 5, 6, 7, 8, 8, 10, 11, 12, 13, 15, 17},
+  {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 1, 1, 1, 1, 1,
+   1, 2, 2, 2, 2, 3, 3, 3, 4, 4, 4, 5, 6, 6, 7, 8, 9, 10, 11, 13, 14, 16, 18, 20, 23, 25}};
+
+static int dbk_is_intra (int t) { return t == ORC_MB_I4x4 || t == ORC_MB_I16x16 || t == ORC_MB_IPCM; }
+static int dbk_is_b (int t) { return t == ORC_MB_B || t == ORC_MB_BSKIP; }
+static int dbk_mv_far (const int32_t* a, const int32_t* b) { return iabs (a[0] - b[0]) >= 4 || iabs (a[1] - b[1]) >= 4; }
+static void dbk_motion (const int32_t* ref, const int32_t* mv, int mb, int blk, int* r, int32_t m[2]) {
+  *r = ref ? ref[16 * mb + blk] : -1;
+  m[0] = *r < 0 ? 0 : mv[32 * mb + 2 * blk];            /* a list that is not used has no vector */
+  m[1] = *r < 0 ? 0 : mv[32 * mb + 2 * blk + 1];
+}
+
+/* 8.7.2.1: bS of the edge between 4x4 block bq of macroblock q and block bp of macroblock p (p == q inside a macroblock) */
+static int dbk_strength (const orc_dbk_pic* d, int q, int bq, int p, int bp, int mb_edge) {
+  const int tq = d->type[q], tp = d->type[p];
+  if (dbk_is_intra (tq) || dbk_is_intra (tp)) return mb_edge ? 4 : 3;
+  /* Reference departure: the inner edges of a skipped macroblock get bS 0 (deblocking.cpp:1184, IS_SKIP).  For P_Skip the
+   * spec agrees (one vector, no coefficients); for B_Skip the spec would derive bS from the direct-mode motion of each block. */
+  if (!mb_edge && (tq == ORC_MB_PSKIP || tq == ORC_MB_BSKIP)) return 0;
+  if (d->nnz[16 * q + bq] || d->nnz[16 * p + bp]) return 2;
+  if (dbk_is_b (tq) || dbk_is_b (tp)) {
+    /* two lists: DeblockingBSliceBsMarginalMBAvcbase (deblocking.cpp:544) / IN_SMB_EDGE_MV (:95).  bS 1 unless both blocks
+     * use the same pair of reference pictures; then the vectors are compared picture by picture, and when both lists of q
+     * name the same picture, both pairings must be far for bS 1 */
+    int rq0, rq1, rp0, rp1;
+    int32_t mq0[2], mq1[2], mp0[2], mp1[2];
+    dbk_motion (d->ref0, d->mv0, q, bq, &rq0, mq0);
+    dbk_motion (d->ref1, d->mv1, q, bq, &rq1, mq1);
+    dbk_motion (d->ref0, d->mv0, p, bp, &rp0, mp0);
+    dbk_motion (d->ref1, d->mv1, p, bp, &rp1, mp1);
+    const int straight = rq0 == rp0 && rq1 == rp1, crossed = rq0 == rp1 && rq1 == rp0;
+    if (!straight && !crossed) return 1;
+    if (rq0 != rq1) return straight ? (dbk_mv_far (mq0, mp0) || dbk_mv_far (mq1, mp1)) : (dbk_mv_far (mq0, mp1) || dbk_mv_far (mq1, mp0));
+    return (dbk_mv_far (mq0, mp0) || dbk_mv_far (mq1, mp1)) && (dbk_mv_far (mq0, mp1) || dbk_mv_far (mq1, mp0));
+  }
+  if (d->compare_refs && d->ref0[16 * q + bq] != d->ref0[16 * p + bp]) return 1;
+  return dbk_mv_far (&d->mv0[32 * q + 2 * bq], &d->mv0[32 * p + 2 * bp]);
+}
+
+/* counts what the edge filter is about to do to one line (the lines of one edge are independent) */
+static void dbk_count_luma (const uint8_t* pix, int sx, int alpha, int beta, int bs, int32_t* st) {
+  const int p0 = pix[-sx], p1 = pix[-2 * sx], p2 = pix[-3 * sx], q0 = pix[0], q1 = pix[sx], q2 = pix[2 * sx];
+  if (!(iabs (p0 - q0) < alpha && iabs (p1 - p0) < beta && iabs (q1 - q0) < beta)) return;
+  st[ORC_DBK_LUMA_BS1 + bs - 1]++;
+  const int ap = iabs (p2 - p0) < beta, aq = iabs (q2 - q0) < beta;
+  if (bs == 4) {
+    if (iabs (p0 - q0) < (alpha >> 2) + 2) { st[ORC_DBK_STRONG]++; st[ORC_DBK_STRONG_AP] += ap; st[ORC_DBK_STRONG_AQ] += aq; }
+  } else {
+    st[ORC_DBK_LT4_AP] += ap; st[ORC_DBK_LT4_AQ] += aq;
+  }
+}
+static void dbk_count_chroma (const uint8_t* pix, int sx, int alpha, int beta, int bs, int32_t* st) {
+  const int p0 = pix[-sx], p1 = pix[-2 * sx], q0 = pix[0], q1 = pix[sx];
+  if (iabs (p0 - q0) < alpha && iabs (p1 - p0) < beta && iabs (q1 - q0) < beta) st[ORC_DBK_CHROMA_BS1 + bs - 1]++;
+}
+
+void orc_deblock_picture (uint8_t* y, uint8_t* cb, uint8_t* cr, int stride_y, int stride_c, int mb_w, int mb_h,
+                          const orc_dbk_pic* d, int32_t* stats) {
+  int32_t dummy[ORC_DBK_NSTATS];
+  int32_t* st = stats ? stats : dummy;
+  for (int mby = 0; mby < mb_h; mby++)
+    for (int mbx = 0; mbx < mb_w; mbx++) {
+      const int q = mby * mb_w + mbx;
+      /* every rule reads the q macroblock's own slice controls */
+      const int idc = d->idc[q], off_a = d->off_a[q], off_b = d->off_b[q];
+      if (idc == 1) { st[ORC_DBK_OFF_IDC1] += 8; continue; }
+      for (int dir = 0; dir < 2; dir++) {                 /* 0: vertical edges (p to the left), 1: horizontal (p above) */
+        const int at_border = dir ? mby == 0 : mbx == 0;
+        const int nb = dir ? q - mb_w : q - 1;
+        for (int e = 0; e < 4; e++) {
+          if (e == 0 && at_border) { st[ORC_DBK_OFF_BORDER]++; continue; }
+          /* idc 2 (deblocking.cpp:671-681): macroblock edges toward another slice stay unfiltered */
+          if (e == 0 && idc == 2 && d->slice[nb] != d->slice[q]) { st[ORC_DBK_OFF_IDC2]++; continue; }
+          /* 8.7: with the 8x8 transform the luma edges at 4 and 12 are no transform block edges */
+          if ((e & 1) && d->t8x8[q]) { st[ORC_DBK_OFF_T8X8]++; continue; }
+          const int p = e == 0 ? nb : q;
+          int bs[4], any = 0;
+          for (int s = 0; s < 4; s++) {
+            const int bq = dir ? 4 * e + s : 4 * s + e;
+            const int bp = dir ? (e == 0 ? 12 + s : bq - 4) : (e == 0 ? 4 * s + 3 : bq - 1);
+            bs[s] = dbk_strength (d, q, bq, p, bp, e == 0);
+            any |= bs[s];
+          }
+          if (!any) continue;
+          /* 8.7.2.2: a macroblock edge uses the mean QP of the two macroblocks (luma and chroma separately) */
+          for (int chroma = 0; chroma < 2; chroma++) {
+            if (chroma && (e & 1)) continue;            /* chroma edges lie at luma edges 0 and 2 */
+            const int32_t* qpa = chroma ? d->qp_c : d->qp;
+            const int qpav = e == 0 ? (qpa[q] + qpa[p] + 1) >> 1 : qpa[q];
+            const int ia = clip3 (qpav + off_a, 0, 51), ib = clip3 (qpav + off_b, 0, 51);
+            const int alpha = kDbkAlpha[ia], beta = kDbkBeta[ib];
+            int8_t tc[4];
+            if (!chroma) {
+              uint8_t* pix = y + (size_t) (16 * mby + (dir ? 4 * e : 0)) * stride_y + 16 * mbx + (dir ? 0 : 4 * e);
+              const int sx = dir ? stride_y : 1, sy = dir ? 1 : stride_y;
+              for (int l = 0; l < 16; l++) if (bs[l >> 2]) dbk_count_luma (pix + l * sy, sx, alpha, beta, bs[l >> 2], st);
+              if (bs[0] == 4) {                           /* bS 4 only on macroblock edges with an intra side: all 4 segments */
+                orc_deblock_luma_eq4 (pix, sx, sy, alpha, beta);
+              } else {
+                for (int s = 0; s < 4; s++) tc[s] = (int8_t) (bs[s] ? kDbkTc0[bs[s] - 1][ia] : -1);
+                orc_deblock_luma_lt4 (pix, sx, sy, alpha, beta, tc);   /* tc = tC0 + ap + aq inside the filter */
+              }
+            } else {
+              const size_t off = (size_t) (8 * mby + (dir ? 2 * e : 0)) * stride_c + 8 * mbx + (dir ? 0 : 2 * e);
+              const int sx = dir ? stride_c : 1, sy = dir ? 1 : stride_c;
+              for (int l = 0; l < 8; l++)
+                if (bs[l >> 1]) {
+                  dbk_count_chroma (cb + off + l * sy, sx, alpha, beta, bs[l >> 1], st);
+                  dbk_count_chroma (cr + off + l * sy, sx, alpha, beta, bs[l >> 1], st);
+                }
+              if (bs[0] == 4) {
+                orc_deblock_chroma_eq4 (cb + off, cr + off, sx, sy, alpha, beta);
+              } else {
+                for (int s = 0; s < 4; s++) tc[s] = (int8_t) (bs[s] ? kDbkTc0[bs[s] - 1][ia] + 1 : 0);   /* chroma: tC = tC0 + 1 */
+                orc_deblock_chroma_lt4 (cb + off, cr + off, sx, sy, alpha, beta, tc);
+              }
+            }
+          }
+        }
+      }
+    }
+}
+
+/* ------------------------------------------------------------------------------------------
  * expand_pic.cpp:40-340,388: replicate the picture border `pad` pixels outwards on all sides
  * ------------------------------------------------------------------------------------------ */
 void orc_expand_plane (uint8_t* pic, int stride, int w, int h, int pad) {

@@ -413,6 +413,28 @@ extern "C" int emu_decode(const uint8_t* bs, long len, uint8_t* out, long cap, i
 }
 
 
+// ---- whole-picture deblocking of given records, the host build of the device filter (deblock_frame_host) ----------------
+// Planes point at sample (0,0); mbi / aux_b hold mb_w * mb_h records as the decoder (dec_mode 1) or the encoder (dec_mode 0)
+// leaves them; aux_b may be NULL.  idc / off_a / off_b: the encoder's per-picture control (the decoder's travels in mbi).
+// tests/test_deblock_oracle_emu.py compares the result with oracle/orc_deblock_picture.
+extern "C" int emu_deblock_picture(uint8_t* y, uint8_t* cb, uint8_t* cr, int stride_y, int stride_c, int mb_w, int mb_h, MbInfo* mbi,
+                                   const DecMbAuxB* aux_b, int dec_mode, int idc, int off_a, int off_b) {
+  if (mb_w < 1 || mb_h < 1 || !mbi || (aux_b && !dec_mode)) return -1;
+  b2h264_build_host_tables();
+  EncFrameParams p;
+  memset(&p, 0, sizeof(p));
+  p.mb_w = mb_w; p.mb_h = mb_h;
+  p.rec_stride_y = stride_y; p.rec_stride_c = stride_c;
+  p.dec_mode = dec_mode; p.dbk_idc = idc; p.dbk_off_a = off_a; p.dbk_off_b = off_b;
+  EncFramePtrs f;
+  memset(&f, 0, sizeof(f));
+  f.rec[0] = y; f.rec[1] = cb; f.rec[2] = cr;
+  f.mbi = mbi;
+  f.dec_aux_b = aux_b;
+  deblock_frame_host(p, f);
+  return 0;
+}
+
 // ---- randomized writer <-> parser round trip (levels up to the Baseline escape range, every macroblock type) -----------
 // Returns 0, a negative ParseError, or 1 + index of the first macroblock that came back different.
 static int random_pictures(unsigned seed, int pictures, bool decodable, uint8_t* stream_out, long cap, long* stream_len);
