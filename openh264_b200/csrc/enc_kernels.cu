@@ -31,6 +31,15 @@ __constant__ uint8_t c_tc0[52][3];
 
 #define DEC_WPC 24         // warps per CTA of the decoder's macroblock kernel (one CTA per SM at 80 registers)
 #define ENC_WPC 23         // WORKER warps per CTA of the encode kernel; one more warp schedules (24 x 32 x 80 registers = one CTA per SM)
+// A full batch of a PULLED list claims up to ENC_PULL x ENC_WPC tasks; a warp that finishes its task takes the next unstarted
+// one of the block (run_stages).  Pulled: A (skip test) and Bs (skip-candidate intra check), bit (stage - 1) of the mask.
+// ENC_PULL = 1 is the plain one-task-per-warp batch.
+#ifndef ENC_PULL
+#define ENC_PULL 2
+#endif
+#ifndef ENC_PULL_LISTS
+#define ENC_PULL_LISTS ((1 << (MBS_A - 1)) | (1 << (MBS_BSKIP - 1)))
+#endif
 
 __device__ __forceinline__ int ld_volatile(const int* p) { return *reinterpret_cast<const volatile int*>(p); }
 
@@ -164,15 +173,19 @@ __device__ __forceinline__ void park_extra(int stage, int* off, int* n) {
 
 // optional batch statistics (debug, B2H264_ENC_STATS): per ready list [batches, tasks, batch cycles]; [NQ] = leader wait cycles
 __device__ unsigned long long g_batch_stats[NQ + 1][3];
-__device__ unsigned long long g_task_wall[NQ][2];                    // per list: cycles from the batch barrier to the end of run_task, tasks
-__device__ unsigned long long g_fill_stats[NQ][ENC_WPC + 1][2];      // per list and batch fill: [batches, cycles]
+// per list: cycles from the batch barrier (a pulled task: from the end of the warp's previous task) to the end of run_task, tasks
+__device__ unsigned long long g_task_wall[NQ][2];
+// per list and batch fill (tasks claimed, up to ENC_PULL x ENC_WPC for a pulled list): [batches, cycles]
+constexpr int kMaxClaim = ENC_PULL * ENC_WPC;
+__device__ unsigned long long g_fill_stats[NQ][kMaxClaim + 1][2];
 extern "C" int b2h264_debug_task_wall(unsigned long long* out, int reset) {
   cudaError_t e = cudaMemcpyFromSymbol(out, g_task_wall, sizeof(g_task_wall));
   if (e == cudaSuccess && reset) { unsigned long long z[NQ][2] = {}; e = cudaMemcpyToSymbol(g_task_wall, z, sizeof(z)); }
   return (int)e;
 }
+// out: NQ x (*wpc + 1) x 2 words, *wpc = the largest batch fill (ENC_PULL x ENC_WPC)
 extern "C" int b2h264_debug_fill_stats(unsigned long long* out, int* n_lists, int* wpc, int reset) {
-  *n_lists = NQ; *wpc = ENC_WPC;
+  *n_lists = NQ; *wpc = kMaxClaim;
   cudaError_t e = cudaMemcpyFromSymbol(out, g_fill_stats, sizeof(g_fill_stats));
   if (reset) { void* a = nullptr; if (cudaGetSymbolAddress(&a, g_fill_stats) == cudaSuccess) cudaMemset(a, 0, sizeof(g_fill_stats)); }
   return (int)e;
@@ -227,6 +240,14 @@ __device__ __forceinline__ void run_task(const StreamFrame* sf, const MbSched& q
 // the list holds two batches' worth); a partial batch only when the workers are already waiting — exactly the decision
 // thread 0 used to take at that moment.  (Experiments that gave up the common start of a batch — warp-asynchronous
 // draws, 2 x 12 and 3 x 8 warp groups — lost more than they saved to instruction-cache misses.)
+// The short stages (A, Bs: ENC_PULL_LISTS) paid the batch barrier, the claim and the slowest warp once per ENC_WPC tasks of
+// ~20 k cycles each.  A full batch of such a list claims up to ENC_PULL x ENC_WPC tasks: every warp starts on task `warp`
+// together as before, then takes the next unstarted task of the block (a shared counter per slot) until the block is
+// empty; the warps drift apart inside the stage, which costs nothing measurable there (DESIGN.md §2).  "The first worker
+// has finished" becomes "a worker found the block empty" (counter > n).  List B stays one task per warp: its
+// re-alignment points (mbk_batch_sync) count the batch's warps.
+static_assert(!(ENC_PULL_LISTS & (1 << (MBS_B - 1))), "stage B's re-alignment barriers need one task per warp");
+static_assert(ENC_PULL >= 1, "a pulled batch holds up to ENC_PULL x ENC_WPC tasks");
 struct BatchSlot { int k, base, n, pad; };
 constexpr int kEncThreads = 32 * (ENC_WPC + 1);
 __device__ __forceinline__ void enc_cta_barrier() { asm volatile("barrier.sync 1, %0;" ::"n"(kEncThreads) : "memory"); }
@@ -234,8 +255,9 @@ __device__ __forceinline__ void enc_cta_barrier() { asm volatile("barrier.sync 1
 template <class Body>
 __device__ __forceinline__ void run_stages(const StreamFrame* sf, int n_streams, const MbSched q, MbScratch& s, int stats, Body body) {
   __shared__ BatchSlot s_slot[2];
-  __shared__ int s_ids[2][ENC_WPC];        // the claimed macroblocks of slot p, read off the ready list by the scheduler warp
-  __shared__ int s_fin[2];                 // workers of the batch in slot p that have finished their macroblock
+  __shared__ int s_ids[2][kMaxClaim];      // the claimed macroblocks of slot p, read off the ready list by the scheduler warp
+  __shared__ int s_fin[2];                 // tasks of the batch in slot p that have finished
+  __shared__ int s_next[2];                // next unstarted task of slot p (starts at the batch's warp count; > n: a warp found it empty)
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int mb_w = sf[0].p.mb_w, mb_h = sf[0].p.mb_h, n_mb = mb_w * mb_h, total = n_streams * n_mb;
   if (warp == ENC_WPC) {
@@ -250,6 +272,8 @@ __device__ __forceinline__ void run_stages(const StreamFrame* sf, int n_streams,
         for (;;) {
           const int fin = run_n ? *reinterpret_cast<volatile int*>(&s_fin[p ^ 1]) : 0;
           const bool all_done = fin >= run_n;
+          // the running batch nears its end: a worker has finished its task (one task per warp) or found the block empty
+          const bool ending = run_n > ENC_WPC ? *reinterpret_cast<volatile int*>(&s_next[p ^ 1]) > run_n : fin > 0;
           if (stats && all_done && !exposed) { exposed = true; t_exposed = clock64(); }
           n_poll++;
           // ONE look at the control words: NQ + 1 independent loads (a line per list), one L2 round trip
@@ -268,14 +292,15 @@ __device__ __forceinline__ void run_stages(const StreamFrame* sf, int n_streams,
             else if (best_avail < ENC_WPC && avail > best_avail) { best = kk; best_avail = avail; }
           }
           const bool full = best_avail >= ENC_WPC;
-          const bool take = best >= 0 && (all_done || (full && (fin > 0 || best_avail >= 2 * ENC_WPC)));
+          const bool take = best >= 0 && (all_done || (full && (ending || best_avail >= 2 * ENC_WPC)));
           if (take) {
             int tail = 0;
 #pragma unroll
             for (int kk = 0; kk < NQ; kk++) if (kk == best) { h = c[kk]; tail = c[NQ + kk]; }
+            const int cap = (ENC_PULL_LISTS >> best) & 1 ? kMaxClaim : ENC_WPC;
             bool got = false;
             for (;;) {                     // a lost race returns the new head: claim from there instead of looking at every list again
-              n = min(ENC_WPC, tail - h);
+              n = min(cap, tail - h);
               if (n <= 0 || (n < ENC_WPC && !all_done)) break;
               const int old = atomicCAS(ctl_head(q, best), h, h + n);
               if (old == h) { got = true; break; }
@@ -287,10 +312,11 @@ __device__ __forceinline__ void run_stages(const StreamFrame* sf, int n_streams,
             continue;
           }
           n_idle++;
-          __nanosleep(all_done ? 100 : fin > 0 ? 400 : 1500);
+          __nanosleep(all_done ? 100 : ending ? 400 : 1500);
         }
         s_slot[p].k = k; s_slot[p].base = h; s_slot[p].n = n;
         s_fin[p] = 0;
+        s_next[p] = min(n, ENC_WPC);
         if (stats) {
           if (exposed) atomicAdd(&g_batch_stats[NQ][2], (unsigned long long)(clock64() - t_exposed));   // what the workers waited for the claim
           atomicAdd(&g_batch_stats[NQ][0], n_poll + (n_fail << 32));        // low word: looks, high word: failed claims
@@ -302,10 +328,10 @@ __device__ __forceinline__ void run_stages(const StreamFrame* sf, int n_streams,
         // lane i fetches the i-th claimed macroblock (its producer may still be writing the entry: spin), so that the workers
         // start from shared memory instead of each paying an L2 round trip after the barrier
         const int kk = s_slot[p].k, nn = s_slot[p].n;
-        if (lane < nn) {
+        for (int i = lane; i < nn; i += 32) {
           int id;
-          while ((id = ld_volatile(q.queue + (size_t)kk * total + s_slot[p].base + lane)) < 0) {}
-          s_ids[p][lane] = id;
+          while ((id = ld_volatile(q.queue + (size_t)kk * total + s_slot[p].base + i)) < 0) {}
+          s_ids[p][i] = id;
         }
       }
       __syncwarp();
@@ -317,31 +343,43 @@ __device__ __forceinline__ void run_stages(const StreamFrame* sf, int n_streams,
     return;
   }
   // ---- workers ----
-  int p = 0, prev_k = -1, prev_n = 0;
+  // One loop and one run_task call site for the first and the pulled tasks: a task loop nested in the batch loop, or k and
+  // n kept in registers across the inlined body, cost the kernel more spills.
+  int p = 0, prev_k = -1, prev_n = 0, t = -1;        // t >= 0: the task of the batch in slot p this warp runs next
   long long t_prev = 0;
   for (;;) {
-    enc_cta_barrier();
-    const int k = s_slot[p].k, n = s_slot[p].n;
-    if (stats && threadIdx.x == 0) {
-      const long long t = clock64();
-      if (prev_k >= 0) {
-        const unsigned long long dt = (unsigned long long)(t - t_prev);     // barrier to barrier: the batch plus whatever the claim left exposed
-        atomicAdd(&g_batch_stats[prev_k][0], 1ull);
-        atomicAdd(&g_batch_stats[prev_k][1], (unsigned long long)prev_n);
-        atomicAdd(&g_batch_stats[prev_k][2], dt);
-        atomicAdd(&g_fill_stats[prev_k][min(prev_n, ENC_WPC)][0], 1ull);
-        atomicAdd(&g_fill_stats[prev_k][min(prev_n, ENC_WPC)][1], dt);
+    if (t < 0) {
+      enc_cta_barrier();
+      if (stats && threadIdx.x == 0) {
+        const long long tc = clock64();
+        if (prev_k >= 0) {
+          const unsigned long long dt = (unsigned long long)(tc - t_prev);  // barrier to barrier: the batch plus whatever the claim left exposed
+          atomicAdd(&g_batch_stats[prev_k][0], 1ull);
+          atomicAdd(&g_batch_stats[prev_k][1], (unsigned long long)prev_n);
+          atomicAdd(&g_batch_stats[prev_k][2], dt);
+          atomicAdd(&g_fill_stats[prev_k][min(prev_n, kMaxClaim)][0], 1ull);
+          atomicAdd(&g_fill_stats[prev_k][min(prev_n, kMaxClaim)][1], dt);
+        }
+        t_prev = tc; prev_k = s_slot[p].k; prev_n = s_slot[p].n;
       }
-      t_prev = t; prev_k = k; prev_n = n;
+      if (s_slot[p].n < 0) break;
+      t = warp;
     }
-    if (n < 0) break;
-    if (warp < n) {
+    const int k = s_slot[p].k, n = s_slot[p].n;
+    if (t < n) {
       const long long t_task = stats ? clock64() : 0;
-      const int id = s_ids[p][warp];
-      run_task(sf, q, s, id, k + 1, mb_w, mb_h, total, n, body);
+      run_task(sf, q, s, s_ids[p][t], k + 1, mb_w, mb_h, total, min(n, ENC_WPC) /* batch_n: warps, not tasks */, body);
+      const int kt = ld_volatile(&s_slot[p].k), nt = ld_volatile(&s_slot[p].n);
       if (lane == 0) atomicAdd(&s_fin[p], 1);
-      if (stats && lane == 0) { atomicAdd(&g_task_wall[k][0], (unsigned long long)(clock64() - t_task)); atomicAdd(&g_task_wall[k][1], 1ull); }
+      if (stats && lane == 0) { atomicAdd(&g_task_wall[kt][0], (unsigned long long)(clock64() - t_task)); atomicAdd(&g_task_wall[kt][1], 1ull); }
+      if (nt > ENC_WPC) {                               // a pulled block: take its next unstarted task
+        int tn = 0;
+        if (lane == 0) tn = atomicAdd(&s_next[p], 1);
+        t = __shfl_sync(MBK_FULL, tn, 0);
+        if (t < nt) continue;
+      }
     }
+    t = -1;                                             // this warp is done with the batch: meet the others at the barrier
     p ^= 1;
   }
 }

@@ -3,12 +3,15 @@
 Why: on the GPU the kernel is bound by its dependency structure (much of the warp time waits at batch barriers), and scheduler variants cost GPU time to try.  This model replays the REAL
 per-macroblock stage paths of the bench clip (recorded by the host build of the macroblock code,
 tools/sim_data/mb_stage_paths_1080p.npy: bit s set = stage s ran; A=1, I=2, Bs=3, B=4, C=5) through the same
-policy — one CTA per SM (132 on an H100), W warps each, a batch = up to W ready tasks of ONE stage, batch time = slowest task + a fixed
-overhead, later stages first, a full batch beats a partial one — with the recorded stage costs
-(tools/enc_stats.py).  The default costs below are the per-task averages tools/enc_stats.py 256 measured on one H100 SXM
-(80 GB HBM3, 400 W power limit, 1,980 MHz max SM clock) before the one-pass refinement / intra check; D is not measured.
+policy — one CTA per SM (132 on an H100), W warps each, a batch = up to W ready tasks of ONE stage, batch time = slowest task
+(body + per-task overhead) + a per-batch overhead, later stages first, a full batch beats a partial one — with the recorded
+stage costs (tools/enc_stats.py, see COST).
 
-usage: python tools/sched_sim.py [--streams 256] [--warps 24] [--variant base|dfill|dfull|half|patience|fastB]
+Variant `pull` models ENC_PULL (enc_kernels.cu, run_stages): a full batch of list A or Bs claims up to pull x W tasks, every
+warp starts one, and each further task goes to the warp that becomes free first; every task notifies its dependants at its
+own end, the batch ends when its last warp does.
+
+usage: python tools/sched_sim.py [--streams 256] [--warps 24] [--variant base|dfill|dfull|half|patience|fastB|pull] [--pull 2]
 """
 import argparse
 import heapq
@@ -19,10 +22,16 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 A, I, BS, B, C, D = 1, 2, 3, 4, 5, 6
-# cycles per task, stage -> cycles: tools/enc_stats.py 256 on an H100 SXM at 400 W (P pictures 1-5 averaged; I = the IDR picture;
-# D = deblocking as a task, a placeholder: in-loop deblocking is a separate kernel)
-COST = {A: 31400, BS: 26500, B: 184000, C: 765000, D: 11200, I: 639000}
-BATCH_OVERHEAD = 3000          # claim + two CTA barriers + park/unpark
+# task body cycles (g_enc_stats), stage -> cycles: tools/enc_stats.py 256 with ENC_PULL = 1, P picture 5, on one H100 80GB HBM3
+# (700 W power limit, 1,980 MHz); I = the stage-I task on the same card; D = deblocking as a task, a placeholder: in-loop
+# deblocking is a separate kernel
+COST = {A: 20200, BS: 15700, B: 131800, C: 235700, D: 11200, I: 206000}
+# same run: per task, task wall (g_task_wall) minus body of stage A = fences, unpark / park, notifications (26.9 k - 20.2 k);
+# per batch, the leader wait (what the workers waited for the claim: 1.72 G cycles over 142 k batches); the slowest-warp tail
+# comes from the task spread.  The model then gives 38.6 ms where the GPU measured 39.0 ms (ENC_PULL = 1), and predicts pull 2
+# at 36.2 ms and pull 3 at 35.2 ms, where the GPU measured 34.2 and 34.5 ms (DESIGN.md §7).
+TASK_OVERHEAD = 6700
+BATCH_OVERHEAD = 12000
 MBW, MBH = 120, 68
 
 
@@ -32,7 +41,7 @@ def build_paths(n_streams, seed=1):
     return [paths[rng.randrange(len(paths))] for _ in range(n_streams)]
 
 
-def simulate(n_streams=256, warps=24, n_cta=132, variant="base", seed=1, cost=None, verbose=False):
+def simulate(n_streams=256, warps=24, n_cta=132, variant="base", seed=1, cost=None, verbose=False, pull=2):
     cost = dict(COST if cost is None else cost)
     if variant == "fastB":
         cost[B] = int(cost[B] * 0.7)
@@ -129,7 +138,7 @@ def simulate(n_streams=256, warps=24, n_cta=132, variant="base", seed=1, cost=No
                     return D, min(gw, a)
                 continue
             if a >= gw:
-                return k, gw
+                return k, min(a, pull * gw) if variant == "pull" and k in (A, BS) else gw
             if a > best_avail:
                 best, best_avail = k, a
         if best is None:
@@ -149,15 +158,23 @@ def simulate(n_streams=256, warps=24, n_cta=132, variant="base", seed=1, cost=No
             tasks = queues[k][heads[k]:heads[k] + n]
             heads[k] += n
             # every warp notifies its dependants as soon as ITS task is done; the group is free after the slowest
-            durs = [int(cost[k] * rng.uniform(0.85, 1.2) * (1.0 if k != B else rng.choice((1.0, 1.0, 1.0, 1.35)))) for _ in tasks]
-            dur = max(durs) + BATCH_OVERHEAD
+            durs = [int(cost[k] * rng.uniform(0.85, 1.2) * (1.0 if k != B else rng.choice((1.0, 1.0, 1.0, 1.35)))) + TASK_OVERHEAD
+                    for _ in tasks]
+            # warp ends: a task more than the group's warps goes to the warp that is free first (only a pulled batch has those)
+            free = [0] * min(n, gw)
+            ends = []
+            for d in durs:
+                j = min(range(len(free)), key=free.__getitem__)
+                free[j] += d
+                ends.append(free[j])
+            dur = max(free) + BATCH_OVERHEAD
             busy_cycles[k] += sum(durs)
             batch_n[k] += 1
             batch_tasks[k] += n
             group_time += dur
-            for t, d in zip(tasks, durs):
+            for t, e in zip(tasks, ends):
                 seq += 1
-                heapq.heappush(ev, (now + d, seq, -1, k, t))
+                heapq.heappush(ev, (now + e, seq, -1, k, t))
             seq += 1
             heapq.heappush(ev, (now + dur, seq, g, k, None))
 
@@ -172,7 +189,7 @@ def simulate(n_streams=256, warps=24, n_cta=132, variant="base", seed=1, cost=No
             dispatch()
     assert coded == total and (not with_d or deblocked == total), (coded, deblocked, total)
     ms = now / 1.965e6
-    res = {"variant": variant, "streams": n_streams, "warps": warps, "kernel_ms": round(ms, 2),
+    res = {"variant": variant + (str(pull) if variant == "pull" else ""), "streams": n_streams, "warps": warps, "kernel_ms": round(ms, 2),
            "group_busy_frac": round(group_time / (now * n_cta * groups), 3),
            "warp_busy_frac": round(sum(busy_cycles.values()) / (now * n_cta * warps), 3),
            "fill": {k: round(batch_tasks[k] / max(1, batch_n[k]), 1) for k in queues if batch_n[k]}}
@@ -184,5 +201,6 @@ if __name__ == "__main__":
     ap.add_argument("--streams", type=int, default=256)
     ap.add_argument("--warps", type=int, default=24)
     ap.add_argument("--variant", default="base")
+    ap.add_argument("--pull", type=int, default=2, help="variant pull: claim up to this many warps' worth of A / Bs tasks")
     a = ap.parse_args()
-    print(simulate(a.streams, a.warps, variant=a.variant))
+    print(simulate(a.streams, a.warps, variant=a.variant, pull=a.pull))
