@@ -17,7 +17,8 @@
  * Supported configuration (everything else is rejected with an error, never silently approximated):
  * CAMERA_VIDEO_REAL_TIME, 1 spatial / 1 temporal layer, RC_OFF_MODE (constant QP), SM_SINGLE_SLICE,
  * CAVLC or CABAC (Baseline / Main / High parameter sets, no 8x8 transform), any iComplexityMode (LOW / MEDIUM / HIGH), 1 reference frame, any loop filter idc / offsets, IDR at the first frame, every uiIntraPeriod frames and on
- * ForceIntraFrame, no denoise / background detection / adaptive quant / scene-change / LTR.
+ * ForceIntraFrame, no denoise / background detection / scene-change / LTR.  (Adaptive quantisation: the reference switches it off
+ * for every configuration, encoder_ext.cpp:300-301, so its output with the flag set is this constant-QP output.)
  * For that configuration the bitstream is bit-identical to the reference's.
  */
 #ifndef B2H264_CODEC_H

@@ -14,8 +14,11 @@
  * stderr; nothing is silently approximated and there is no CPU fallback):
  *   iUsageType CAMERA_VIDEO_REAL_TIME, iSpatialLayerNum 1, iTemporalLayerNum 1, iRCMode RC_OFF_MODE,
  *   SM_SINGLE_SLICE, iEntropyCodingModeFlag 0, iNumRefFrame 1 or AUTO, uiIntraPeriod 0, iLoopFilterDisableIdc 0
- *   with zero offsets, iComplexityMode MEDIUM/HIGH, bEnableDenoise / BackgroundDetection / AdaptiveQuant /
+ *   with zero offsets, iComplexityMode MEDIUM/HIGH, bEnableDenoise / BackgroundDetection /
  *   SceneChangeDetect / LongTermReference / FrameSkip all false, bEnableFrameCroppingFlag true,
+ *   bEnableAdaptiveQuant either way with any iMinQp / iMaxQp (the reference's ParamValidation switches adaptive
+ *   quantisation off for every configuration, encoder_ext.cpp:300-301: the bitstream is the constant-QP one and
+ *   GetOption(ENCODER_OPTION_SVC_ENCODE_PARAM_EXT) reports it off, as the reference's does),
  *   profile baseline/unknown, no SSEI / simulcast / prefix NAL, eSpsPpsIdStrategy CONSTANT_ID or INCREASING_ID
  *   (every IDR's parameter sets take the next id, as in the reference), width % 4 == 0, height % 2 == 0.
  * Initialize(SEncParamBase*) implies RC on (the reference's default RC_QUALITY_MODE): unsupported unless

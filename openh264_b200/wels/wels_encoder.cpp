@@ -45,12 +45,12 @@ class B2Encoder : public ISVCEncoder {
     e.sSpatialLayers[0].fFrameRate = p->fMaxFrameRate;
     e.sSpatialLayers[0].iSpatialBitrate = p->iTargetBitrate;
     // ParamBaseTranscode keeps FillDefault's tools switched on: scene-change detection (inserts IDRs), background
-    // detection (changes the skip decision), adaptive quantisation (per-MB QP even with RC off: WelsRcMbInitDisable,
-    // ratectl.cpp:1301), frame skipping, and LOW_COMPLEXITY mode decision.  None of them is a no-op for the output,
-    // so this entry point cannot be honoured bit-exactly; it is refused with the reason instead of approximated.
+    // detection (changes the skip decision), frame skipping, and LOW_COMPLEXITY mode decision.  The first two are not
+    // no-ops for the output, so this entry point cannot be honoured bit-exactly; it is refused with the reason instead
+    // of approximated.  (Adaptive quantisation, also on by default, is not among them: see InitializeExt.)
     if (p->iRCMode != RC_OFF_MODE) { why("Initialize(SEncParamBase): rate control is on (only RC_OFF_MODE; needs the on-device bit count)"); return cmUnsupportedData; }
-    why("Initialize(SEncParamBase) implies bEnableSceneChangeDetect, bEnableBackgroundDetection, bEnableAdaptiveQuant and "
-        "iComplexityMode = LOW_COMPLEXITY, which change the bitstream; use InitializeExt with them off");
+    why("Initialize(SEncParamBase) implies bEnableSceneChangeDetect and bEnableBackgroundDetection, which change the bitstream; "
+        "use InitializeExt with them off");
     (void)e;
     return cmUnsupportedData;
   }
@@ -69,8 +69,11 @@ class B2Encoder : public ISVCEncoder {
         p->iLoopFilterBetaOffset < -6 || p->iLoopFilterBetaOffset > 6) return cmInitParaError;       // encoder_ext.cpp:316-323
     REQUIRE(p->iComplexityMode == LOW_COMPLEXITY || p->iComplexityMode == MEDIUM_COMPLEXITY || p->iComplexityMode == HIGH_COMPLEXITY,
             "iComplexityMode");
-    REQUIRE(!p->bEnableDenoise && !p->bEnableBackgroundDetection && !p->bEnableAdaptiveQuant && !p->bEnableSceneChangeDetect,
-            "denoise / background detection / adaptive quant / scene change detection enabled");
+    // bEnableAdaptiveQuant is accepted and has no effect, as in the reference: its ParamValidation switches it off for every
+    // configuration (encoder_ext.cpp:300-301, "turn off adaptive quant now"), so the bitstream is the constant-QP one and the
+    // resolved parameters report it off.  iMinQp / iMaxQp only bound rate control, which is off here.
+    REQUIRE(!p->bEnableDenoise && !p->bEnableBackgroundDetection && !p->bEnableSceneChangeDetect,
+            "denoise / background detection / scene change detection enabled");
     REQUIRE(!p->bEnableLongTermReference && !p->bEnableFrameSkip, "LTR or frame skip enabled");
     REQUIRE(p->bEnableFrameCroppingFlag, "bEnableFrameCroppingFlag false");
     REQUIRE(!p->bEnableSSEI && !p->bSimulcastAVC && !p->bPrefixNalAddingCtrl, "SSEI / simulcast / prefix NAL");
@@ -110,6 +113,7 @@ class B2Encoder : public ISVCEncoder {
     // what GetOption(ENCODER_OPTION_SVC_ENCODE_PARAM_EXT) reports is the RESOLVED configuration, as with the reference
     // (param_svc.h:370-372, encoder_ext.cpp:126-141,652-664)
     if (par_.uiIntraPeriod == (unsigned int)-1) par_.uiIntraPeriod = 0;
+    par_.bEnableAdaptiveQuant = false;
     {
       EProfileIdc& pr = par_.sSpatialLayers[0].uiProfileIdc;
       if (pr != PRO_BASELINE && pr != PRO_MAIN && pr != PRO_HIGH) pr = PRO_UNKNOWN;
