@@ -111,8 +111,8 @@ int  b2h264_enc_set_stream (b2h264_enc* e, void* stream);
  * Replaces, for Baseline / Main / High streams with CAVLC or CABAC slice data (I and P slices, several slices per picture in raster
  * order, up to 16 reference frames with list modification, sliding-window and memory-management marking incl. long-term pictures,
  * all partition shapes down to 4x4, I_PCM, constrained intra prediction, per-slice deblocking control, non-reference pictures, B slices with
- * spatial / temporal direct prediction and implicit weights, the 8x8 transform with Intra_8x8, explicit weights in P slices, a chroma QP
- * offset; no FMO / ASO, explicit weights in B slices, interlace, scaling lists, SVC extensions), ISVCDecoder::DecodeFrameNoDelay
+ * spatial / temporal direct prediction and implicit weights, the 8x8 transform with Intra_8x8, explicit weights in P and B slices, a
+ * chroma QP offset; no FMO / ASO, interlace, scaling lists, SVC extensions), ISVCDecoder::DecodeFrameNoDelay
  * (codec/api/wels/codec_api.h:383; codec/decoder/plus/src/welsDecoderExt.cpp:~700).  The host parses, the GPU
  * reconstructs, deblocks and pads.  Anything else is rejected: -101 truncated, -102 unsupported stream feature,
  * -103 invalid syntax, -104 slice before its parameter sets, -105 the slices given do not cover the picture; -2 picture size differs from the configuration. */

@@ -11,6 +11,7 @@
 #pragma once
 #include "enc_inter.cuh"
 #include "dec_t8x8.cuh"
+#include "wp_formula.h"
 
 namespace mbk {
 
@@ -140,16 +141,16 @@ MBK_FN void dec_i8x8_blocks(MbScratch& s, const MbOut& m, int nb_i, int qp) {
 // its registers and stack frame.
 MBK_FN void dec_b_mb(const MbCtx& c, const EncFrameParams& p, MbScratch& s, const MbOut& m, const DecMbAux& aux, int mbx, int mby,
                      uint8_t* pl, uint8_t* pc, int qp) {
-  // B macroblock (GetInterBPred, rec_mb.cpp:462 ff.): the parser resolved both lists (h264_motion.h) — per 8x8 a picture slot and
+  // B macroblock (GetInterBPred, rec_mb.cpp:666 ff.): the parser resolved both lists (h264_motion.h) — per 8x8 a picture slot and
   // FINAL vectors per 4x4 block for list 0 (aux) and list 1 (dec_aux_b).  Each list is motion compensated like a P partition (one
-  // 8x8 where the four blocks move together, else 4x4 by 4x4); where both lists predict, the two predictions are combined with the
-  // 8x8's weights (32 / 32: the plain average (a + b + 1) >> 1; implicit weights otherwise, 8.4.2.3 with logWD 5 and no offsets).
+  // 8x8 where the four blocks move together, else 4x4 by 4x4), then the 8x8 goes through the weighting formula its record names
+  // (DecMbAuxB: one list, two lists, or none; default, implicit and explicit weights are all values of the same two formulas).
   const DecMbAuxB& ab = c.f.dec_aux_b[mby * p.mb_w + mbx];
   uint8_t* pl1 = s.pred_y[1];
   uint8_t* pc1 = s.pred_c[1];
   for (int k = 0; k < 4; k++) {
-    const int use = ab.pred_lists[k];                            // lists that enter the sample prediction (see DecMbAuxB)
-    const int r0 = (use & 1) ? aux.ref_idx[k] : -1, r1 = (use & 2) ? ab.ref_idx[k] : -1;
+    const int pred = ab.pred[k];
+    const int r0 = (pred & DECB_L0) ? aux.ref_idx[k] : -1, r1 = (pred & DECB_L1) ? ab.ref_idx[k] : -1;
     bool whole = true;
     for (int j = 1; j < 4; j++)
       whole = whole && aux.mvd[4 * k + j][0] == aux.mvd[4 * k][0] && aux.mvd[4 * k + j][1] == aux.mvd[4 * k][1] &&
@@ -169,27 +170,27 @@ MBK_FN void dec_b_mb(const MbCtx& c, const EncFrameParams& p, MbScratch& s, cons
         }
       }
     }
-    if (ab.wp_on && (r0 >= 0) != (r1 >= 0)) {
-      // explicit weights of the 8x8's single reference (WeightPrediction, rec_mb.cpp:298; 8.4.2.3.2): luma, then Cb / Cr
-      const int qx = (k & 1) * 8, qy = (k >> 1) * 8;
+    if (pred & (DECB_WEIGHT | DECB_BI)) {
+      // the 8x8's samples, luma then Cb / Cr: first input from buffer 0, second from buffer 1 where both lists were motion compensated,
+      // else from buffer 0 as well; the one-list formula may cover the lower 8x4 / right 4x8 only (DECB_LOWER / DECB_RIGHT)
+      const bool bi = (pred & DECB_BI) != 0, two = r0 >= 0 && r1 >= 0;
+      const int qx = (k & 1) * 8, qy = (k >> 1) * 8, x0 = (pred & DECB_RIGHT) ? 4 : 0, y0 = (pred & DECB_LOWER) ? 4 : 0;
       for (int i = lane_id(); i < 64 + 32; i += MBK_WS) {
-        int pos, plane;
-        uint8_t* a;
-        if (i < 64) { pos = (qy + (i >> 3)) * 16 + qx + (i & 7); a = pl; plane = 0; }
-        else { const int t = i - 64, cpl = t >> 4, e = t & 15; pos = 64 * cpl + ((qy >> 1) + (e >> 2)) * 8 + (qx >> 1) + (e & 3); a = pc; plane = 1 + cpl; }
-        const int ld = ab.wp_log2[plane ? 1 : 0], w = ab.wp[k][plane][0], o = ab.wp[k][plane][1];
-        a[pos] = (uint8_t)clip255(ld >= 1 ? ((a[pos] * w + (1 << (ld - 1))) >> ld) + o : a[pos] * w + o);
-      }
-      warp_sync();
-    }
-    if (r0 >= 0 && r1 >= 0) {
-      const int w1 = ab.w1[k], w0 = 64 - w1, qx = (k & 1) * 8, qy = (k >> 1) * 8;
-      for (int i = lane_id(); i < 64 + 32; i += MBK_WS) {
-        int pos;
+        int pos, plane, x, y;
         uint8_t *a, *b;
-        if (i < 64) { pos = (qy + (i >> 3)) * 16 + qx + (i & 7); a = pl; b = pl1; }
-        else { const int t = i - 64, cpl = t >> 4, e = t & 15; pos = 64 * cpl + ((qy >> 1) + (e >> 2)) * 8 + (qx >> 1) + (e & 3); a = pc; b = pc1; }
-        a[pos] = (uint8_t)clip255((a[pos] * w0 + b[pos] * w1 + 32) >> 6);
+        if (i < 64) { x = i & 7; y = i >> 3; pos = (qy + y) * 16 + qx + x; a = pl; b = two ? pl1 : pl; plane = 0; }
+        else {
+          const int t = i - 64, cpl = t >> 4;
+          x = 2 * (t & 3); y = 2 * ((t & 15) >> 2);                 // chroma sample in luma units of the 8x8, for the region test
+          pos = 64 * cpl + ((qy + y) >> 1) * 8 + ((qx + x) >> 1); a = pc; b = two ? pc1 : pc; plane = 1 + cpl;
+        }
+        if (x < x0 || y < y0) continue;
+        const int e = 4 * plane + k, ld = (aux.wp_log2 >> (plane ? 4 : 0)) & 15;
+        const int v = bi ? wp_bi(a[pos], b[pos], ab.w0[e], ab.w1[e], ab.o[e], ld) : wp_single(a[pos], ab.w0[e], ab.o[e], ld);
+#ifdef B2H264_WP_STATS
+        if ((aux.flags & DECAUX_EXPLICIT_B) && (v < 0 || v > 255)) b2h264_wp_stat(v < 0 ? WPS_CLIP_LOW : WPS_CLIP_HIGH, 1);
+#endif
+        a[pos] = (uint8_t)clip255(v);
       }
       warp_sync();
     }

@@ -61,35 +61,42 @@ typedef struct {
  * One record per macroblock next to the MbOut array (h264_parse.h -> dec_mb.cuh / enc_deblock.cuh). */
 typedef struct {
   uint8_t avail;                          // NB_LEFT | NB_TOP | NB_TOPLEFT | NB_TOPRIGHT: neighbours in the SAME slice (6.4.x availability)
-  uint8_t flags;                          // bit 0: sub_type / mvd[16] below are used; bit 1: constrained_intra_pred_flag
+  uint8_t flags;                          // DECAUX_* below
   uint8_t dbk_idc;                        // disable_deblocking_filter_idc of the macroblock's slice
   int8_t  alpha_off, beta_off;            // FilterOffsetA / FilterOffsetB (already x2)
-  uint8_t pad;
-  uint16_t slice;                         // slice number inside the picture
+  uint8_t wp_log2;                        // macroblocks with a DecMbAuxB record: ld of its weighting formula, luma bits 0-3, chroma 4-7
+  uint16_t slice;                        // slice number inside the picture
   uint8_t sub_type[4];                    // per 8x8: 0 8x8, 1 8x4, 2 4x8, 3 4x4
   int8_t  ref_idx[4];                     // per 8x8: PICTURE SLOT of its reference picture (the parser resolves RefPicList0)
   int16_t mvd[16][2];                     // sub-macroblock partition j of 8x8 k at [4 * k + j]
 } DecMbAux;                               // 16 + 64 = 80 bytes
-/* Decoder, B slices only: list 1 of a macroblock (one record per macroblock, uploaded only for pictures that hold B slices).
- * For a B macroblock DecMbAux::ref_idx / mvd hold list 0 the same way: picture slot per 8x8 (-1: list not used) and the FINAL vector
- * of 4x4 block j of 8x8 k at [4 * k + j] (coding order), not a difference. */
+/* Decoder: list 1 and the sample weighting of a macroblock that travels resolved (a B macroblock, or a P macroblock of a slice with
+ * explicit weights); one record per macroblock, uploaded only for pictures that hold such macroblocks.  For these DecMbAux::ref_idx /
+ * mvd hold list 0 the same way: picture slot per 8x8 (-1: list not used) and the FINAL vector of 4x4 block j of 8x8 k at [4 * k + j]
+ * (coding order), not a difference.
+ * The sample prediction of 8x8 k is its motion-compensated lists (pred[k] bits 0 / 1) put through one of the two formulas of
+ * wp_formula.h with w0 / w1 / o at [4 * plane + k] (plane Y, Cb, Cr) and ld from DecMbAux::wp_log2: the one-list formula
+ * (DECB_WEIGHT: w0, o), the two-list formula (DECB_BI: w0, w1, o), or neither (the prediction as it is).  Default averaging is ld 0
+ * with weights 1 / 1, implicit weights ld 5 with w0 = 64 - w1, explicit weights the table's values (two lists: o = (o0 + o1 + 1) >> 1).
+ * ref_idx and mv sit where the deblocking filter reads them (enc_deblock.cuh). */
 typedef struct {
   int8_t  ref_idx[4];                     // per 8x8: picture slot of the list-1 reference, -1: list 1 not used
-  uint8_t pred_lists[4];                  // per 8x8: lists that enter the SAMPLE prediction (bit 0 / bit 1).  Normally the lists in use; the
-                                          // reference's GetInterBPred (rec_mb.cpp:737-825) predicts a bi-predicted 16x8 / 8x16 partition from
-                                          // one list only (first partition: list 1, second: list 0) and its output is the oracle
-  int16_t w1[4];                          // per 8x8 with both lists: weight of the list-1 prediction out of 64 (32: plain average; implicit
-                                          // weights 8.4.2.3.1 otherwise); w0 = 64 - w1
+  int8_t  o[12];                          // offset of the weighting formula, plane p / 8x8 k at [4 * p + k]
   int16_t mv[16][2];                      // final list-1 vector of 4x4 block j of 8x8 k at [4 * k + j]
-  uint8_t wp_on;                          // explicit weights (pred_weight_table of the slice) apply to this macroblock's single-list predictions
-  uint8_t wp_log2[2];                     // luma_log2_weight_denom, chroma_log2_weight_denom
-  uint8_t pad;
-  int16_t wp[4][3][2];                    // per 8x8, plane Y / Cb / Cr: weight, offset of its (single) reference
-} DecMbAuxB;                              // 132 bytes
+  int16_t w0[12], w1[12];                 // weights of the formula's first / second input, [4 * p + k]
+  uint8_t pred[4];                        // per 8x8: DECB_* below
+} DecMbAuxB;                              // 4 + 12 + 64 + 48 + 4 = 132 bytes
+#define DECB_L0 1                         /* list 0 is motion compensated into prediction buffer 0 */
+#define DECB_L1 2                         /* list 1 is motion compensated: into buffer 1 next to list 0, else into buffer 0 */
+#define DECB_WEIGHT 4                     /* one-list formula on buffer 0 */
+#define DECB_BI 8                         /* two-list formula on buffers 0 and 1, on buffer 0 twice when one list is motion compensated */
+#define DECB_LOWER 16                     /* DECB_WEIGHT covers the lower 8x4 of the 8x8 only (see emit_resolved, h264_motion.h) */
+#define DECB_RIGHT 32                     /* DECB_WEIGHT covers the right 4x8 of the 8x8 only */
 #define DECAUX_SUB 1
 #define DECAUX_CIP 2
 #define DECAUX_T8 4                       /* transform_size_8x8_flag: the luma levels are four 8x8 blocks (MbOut::luma[4k .. 4k+3] = 64 levels in
                                              8x8 zig-zag order); an MBT_I4x4 record with this flag is an Intra_8x8 macroblock (prev / rem flags [0..3]) */
+#define DECAUX_EXPLICIT_B 8               /* a macroblock of a B slice with explicit weights (weighted_bipred_idc 1) */
 
 #define MBOUT_HEADER_WORDS 20             /* mb_type .. nnz: all a P_SKIP macroblock needs to hand over */
 

@@ -13,6 +13,7 @@
 #include <string.h>
 
 #include "h264_parse.h"
+#include "wp_formula.h"
 
 namespace b2h264 {
 
@@ -26,6 +27,7 @@ struct WpTable {
   bool on = false;
   int log2[2] = {0, 0};                          // luma, chroma denominators
   int16_t w[2][32][3][2];
+  uint8_t given[2][32];                          // luma_weight_flag (bit 0), chroma_weight_flag (bit 1): 0 = the default weight and offset
 };
 
 // what a B slice adds to the slice state
@@ -35,6 +37,7 @@ struct BSliceCtx {
   int n_ref[2] = {0, 0};
   RefEntry list[2][33];
   int implicit = 0;                              // weighted_bipred_idc == 2
+  const WpTable* wp = nullptr;                   // weighted_bipred_idc == 1: the slice's pred_weight_table
   const MotionStore* col = nullptr;              // motion field of RefPicList1[0]
   bool col_long_term = false;
   bool cabac = false;                            // entropy coder of the slice: the reference's two parsers treat temporal-direct 8x8s differently
@@ -339,14 +342,20 @@ inline bool derive_b(MotionCtx& M, int idx, int avail, const BMbSyntax& sx, cons
     for (int l = 0; l < 2; l++)
       for (int k = 0; k < 4; k++)
         if (sx.sub[k] == 0) M.set(l, (k & 1) * 2, (k >> 1) * 2, 2, 2, dref[l][k], dmv[l][k][0], dmv[l][k][1]);
-  if (!emit_resolved(M, sx, S, nullptr, ax, axb)) return false;
+  if (!emit_resolved(M, sx, S, S.wp, ax, axb)) return false;
   M.store(idx, S.list[0], S.list[1]);
   return true;
 }
 
-// the macroblock's cells -> hand-over records: picture slots per 8x8, final vectors in coding order, weights
+// the macroblock's cells -> hand-over records: picture slots per 8x8, final vectors in coding order, and how each 8x8 forms its sample
+// prediction (DecMbAuxB: the lists that are motion compensated, the weighting formula and its weights).  `wp`: explicit weights of the
+// slice (pred_weight_table of a P slice with weighted_pred_flag or a B slice with weighted_bipred_idc 1), else NULL.
 inline bool emit_resolved(const MotionCtx& M, const BMbSyntax& sx, const BSliceCtx& S, const WpTable* wp, DecMbAux* ax, DecMbAuxB* axb) {
-  axb->wp_on = 0;
+  const bool ex = wp && wp->on;
+  const int ld[2] = {ex ? wp->log2[0] : S.implicit ? 5 : 0, ex ? wp->log2[1] : S.implicit ? 5 : 0};
+  ax->wp_log2 = (uint8_t)(ld[0] | ld[1] << 4);
+  const bool explicit_b = ex && S.n_ref[1] > 0;
+  if (explicit_b) ax->flags |= DECAUX_EXPLICIT_B;
   for (int k = 0; k < 4; k++) {
     const int c0 = MotionCtx::cell((k & 1) * 2, (k >> 1) * 2);
     int r[2];
@@ -362,29 +371,76 @@ inline bool emit_resolved(const MotionCtx& M, const BMbSyntax& sx, const BSliceC
         d[0] = r[l] < 0 ? 0 : M.mvc[l][c][0]; d[1] = r[l] < 0 ? 0 : M.mvc[l][c][1];
       }
     }
-    int w1 = 32;
-    if (S.implicit && r[0] >= 0 && r[1] >= 0) {                    // implicit weights (8.4.2.3.1)
-      const RefEntry& e0 = S.list[0][r[0]];
-      const RefEntry& e1 = S.list[1][r[1]];
-      int dsf;
-      if (dist_scale(S.cur_poc, e0.poc, e1.poc, e0.lt || e1.lt, &dsf) && (dsf >> 2) >= -64 && (dsf >> 2) <= 128) w1 = dsf >> 2;
-    }
-    axb->w1[k] = (int16_t)w1;
-    int use = (r[0] >= 0 ? 1 : 0) | (r[1] >= 0 ? 2 : 0);
+    const int lists = (r[0] >= 0 ? 1 : 0) | (r[1] >= 0 ? 2 : 0);
+    // The reference's GetInterBPred (rec_mb.cpp:737-827) motion compensates both lists of a two-list 16x8 / 8x16 partition into the
+    // same destination before it combines that destination with the list-1 prediction of the second buffer, and advances the
+    // destination of the second partition twice.  So the FIRST partition is the two-list formula on its list-1 prediction twice
+    // (weights of refIdxL0 and refIdxL1: with default or implicit weights, or any w0 + w1 = 2^(ld + 1) and no offsets, that is the
+    // list-1 prediction itself), and the SECOND is its list-0 prediction, unweighted: the combined samples land outside the macroblock
+    // and the one-list weighting only runs for one-list partitions.  The vectors and reference indices stay as coded (neighbours'
+    // prediction, direct modes, the filter).
+    int quirk = 0;                                                 // 1 / 2: first / second such partition
     if (!sx.skip && sx.type >= 4 && sx.type <= 21) {
-      // the reference predicts a bi-predicted partition of a 16x8 / 8x16 macroblock from ONE list (GetInterBPred, rec_mb.cpp:737-825: both
-      // lists are motion compensated into the same destination before the "average" with the second buffer, and the destination pointer
-      // of the second partition is advanced twice): the first partition ends up as its list-1 prediction, the second as its list-0
-      // prediction.  The vectors and reference indices stay as coded (neighbours' prediction, direct modes, the filter).
       const int part = b_is_16x8(sx.type) ? (k >> 1) : (k & 1);
-      if (b_part_lists(sx.type, part) == 3) use = part == 0 ? 2 : 1;
+      if (b_part_lists(sx.type, part) == 3) quirk = part + 1;
     }
-    axb->pred_lists[k] = (uint8_t)use;
-    if (wp && wp->on && (use == 1 || use == 2)) {                  // explicit weights of the 8x8's reference (8.4.2.3.2, one list)
-      const int l = use - 1;
-      axb->wp_on = 1; axb->wp_log2[0] = (uint8_t)wp->log2[0]; axb->wp_log2[1] = (uint8_t)wp->log2[1];
-      for (int pl = 0; pl < 3; pl++) { axb->wp[k][pl][0] = wp->w[l][r[l]][pl][0]; axb->wp[k][pl][1] = wp->w[l][r[l]][pl][1]; }
+    // A one-list 8x4 / 4x8 sub-macroblock of B_8x8: the reference weights its second half only (WeightPrediction runs once, after the
+    // destination was advanced to the second sub-macroblock partition, rec_mb.cpp:934-944, :977-987).
+    const bool direct = sx.skip || sx.type == 0 || (sx.type == 22 && sx.sub[k] == 0);
+    const int shape = (sx.type == 22 && !direct && b_sub_lists(sx.sub[k]) != 3) ? b_sub_shape(sx.sub[k]) : 0;
+    int pred = quirk == 1 ? (ex ? DECB_L1 | DECB_BI : DECB_L1) : quirk == 2 ? DECB_L0 : lists;
+    if (lists == 3 && !quirk) pred |= DECB_BI;
+    if (ex && lists != 3) pred |= DECB_WEIGHT | (shape == 1 ? DECB_LOWER : shape == 2 ? DECB_RIGHT : 0);
+    axb->pred[k] = (uint8_t)pred;
+    for (int pl = 0; pl < 3; pl++) {
+      int w0 = 0, w1 = 0, o = 0;
+      if ((pred & DECB_BI) && ex) {                                // explicit weights (8.4.2.3.2)
+        w0 = wp->w[0][r[0]][pl][0]; w1 = wp->w[1][r[1]][pl][0];
+        o = wp_bi_offset(wp->w[0][r[0]][pl][1], wp->w[1][r[1]][pl][1]);
+      } else if (pred & DECB_BI) {                                 // implicit weights (8.4.2.3.1), else the plain average
+        w1 = S.implicit ? 32 : 1;
+        const RefEntry& e0 = S.list[0][r[0]];
+        const RefEntry& e1 = S.list[1][r[1]];
+        int dsf;
+        if (S.implicit && dist_scale(S.cur_poc, e0.poc, e1.poc, e0.lt || e1.lt, &dsf) && (dsf >> 2) >= -64 && (dsf >> 2) <= 128) w1 = dsf >> 2;
+        w0 = S.implicit ? 64 - w1 : 1;
+      } else if (pred & DECB_WEIGHT) {
+        const int l = (pred & DECB_L0) ? 0 : 1;
+        w0 = wp->w[l][r[l]][pl][0]; o = wp->w[l][r[l]][pl][1];
+      }
+      axb->w0[4 * pl + k] = (int16_t)w0; axb->w1[4 * pl + k] = (int16_t)w1; axb->o[4 * pl + k] = (int8_t)o;
     }
+#ifdef B2H264_WP_STATS
+    if (explicit_b) {                                              // coverage counters (host build only, wp_formula.h)
+      if (quirk) {
+        const int sum = wp->w[0][r[0]][0][0] + wp->w[1][r[1]][0][0];
+        if (sum != 1 << (ld[0] + 1) && (wp->w[0][r[0]][0][1] | wp->w[1][r[1]][0][1])) b2h264_wp_stat(quirk == 1 ? WPS_QUIRK_FIRST : WPS_QUIRK_SECOND, 1);
+      }
+      if (lists != 3) b2h264_wp_stat(lists == 1 ? WPS_SINGLE_L0 : WPS_SINGLE_L1, 1);
+      else if (!direct) b2h264_wp_stat(sx.type == 3 ? WPS_BI_16x16 : b_is_16x8(sx.type) ? WPS_BI_16x8 : b_is_8x16(sx.type) ? WPS_BI_8x16 : WPS_BI_SUB, 1);
+      if (direct) b2h264_wp_stat(S.direct_spatial ? WPS_SPATIAL_DIRECT : WPS_TEMPORAL_DIRECT, 1);
+      if (sx.skip) b2h264_wp_stat(WPS_B_SKIP, 1);
+      if (shape == 1 || shape == 2) b2h264_wp_stat(WPS_HALF, 1);
+      if (quirk != 2) {                                            // the table entries whose values enter the samples
+        for (int l = 0; l < 2; l++) {
+          if (r[l] < 0) continue;
+          if (r[l] > 0) b2h264_wp_stat(l ? WPS_REF_L1_GT0 : WPS_REF_L0_GT0, 1);
+          if (wp->given[l][r[l]] != 3) b2h264_wp_stat(WPS_DEFAULTED, 1);
+          for (int pl = 0; pl < 3; pl++) {
+            const int w = wp->w[l][r[l]][pl][0], o = wp->w[l][r[l]][pl][1];
+            if (w == -128) b2h264_wp_stat(WPS_WEIGHT_MIN, 1);
+            if (w == 127) b2h264_wp_stat(WPS_WEIGHT_MAX, 1);
+            if (o == -128) b2h264_wp_stat(WPS_OFFSET_MIN, 1);
+            if (o == 127) b2h264_wp_stat(WPS_OFFSET_MAX, 1);
+          }
+        }
+        if (ld[0] == 0) b2h264_wp_stat(WPS_DENOM_Y0, 1);
+        if (ld[0] == 7) b2h264_wp_stat(WPS_DENOM_Y7, 1);
+        if (ld[1] == 0) b2h264_wp_stat(WPS_DENOM_C0, 1);
+        if (ld[1] == 7) b2h264_wp_stat(WPS_DENOM_C7, 1);
+      }
+    }
+#endif
   }
   return true;
 }

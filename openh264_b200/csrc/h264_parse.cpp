@@ -7,6 +7,7 @@
 #include <stddef.h>
 #include <string.h>
 
+
 #include "cavlc_tables.h"
 #include "h264_cabac_dec.h"
 #include "h264_motion.h"
@@ -527,12 +528,15 @@ int parse_slice(BitReader& r, const Nal& nal, ParserState* st, ParsedPicture* pi
     for (int l = 0; l < (is_b ? 2 : 1); l++)
       for (int i = 0; i < (l ? n_ref1 : n_ref); i++) {
         for (int pl = 0; pl < 3; pl++) { wp.w[l][i][pl][0] = (int16_t)(1 << wp.log2[pl ? 1 : 0]); wp.w[l][i][pl][1] = 0; }
-        if (r.bit()) {
+        const int luma_flag = r.bit();
+        if (luma_flag) {
           const int w = r.se(), o = r.se();
           if (w < -128 || w > 127 || o < -128 || o > 127) return PARSE_INVALID;
           wp.w[l][i][0][0] = (int16_t)w; wp.w[l][i][0][1] = (int16_t)o;
         }
-        if (r.bit())
+        const int chroma_flag = r.bit();
+        wp.given[l][i] = (uint8_t)(luma_flag | chroma_flag << 1);
+        if (chroma_flag)
           for (int pl = 1; pl < 3; pl++) {
             const int w = r.se(), o = r.se();
             if (w < -128 || w > 127 || o < -128 || o > 127) return PARSE_INVALID;
@@ -540,7 +544,6 @@ int parse_slice(BitReader& r, const Nal& nal, ParserState* st, ParsedPicture* pi
           }
       }
     if (!r.ok()) return PARSE_TRUNCATED;
-    if (is_b) return PARSE_UNSUPPORTED;                       // explicit weights in B slices (weighted_bipred_idc 1) are not built
     if (st->profile == 66) return PARSE_INVALID;
   }
   const bool is_ref = nal.ref_idc != 0;                       // a non-reference picture is output but never predicted from
@@ -641,6 +644,7 @@ int parse_slice(BitReader& r, const Nal& nal, ParserState* st, ParsedPicture* pi
     bsl.direct_spatial = direct_spatial; bsl.cur_poc = poc; bsl.n_ref[0] = n_ref; bsl.n_ref[1] = n_ref1;
     for (int l = 0; l < 2; l++) for (int i = 0; i < 33; i++) bsl.list[l][i] = lists[l][i];
     bsl.implicit = st->weighted_bipred_idc == 2;
+    bsl.wp = wp.on ? &wp : nullptr;
     bsl.cabac = st->entropy_cabac;
     const int cslot = lists[1][0].slot;
     bsl.col = (cslot >= 0 && cslot < (int)st->motion.size()) ? &st->motion[cslot] : nullptr;
@@ -1278,3 +1282,16 @@ int probe_access_unit(const uint8_t* au, size_t len, int* width, int* height, in
 }
 
 }  // namespace b2h264
+
+#ifdef B2H264_WP_STATS
+// coverage counters of explicit weighted prediction in B slices (WPS_* in wp_formula.h; the host build decodes on one thread)
+static long long g_wp_stats[WPS_N];
+void b2h264_wp_stat(int which, long long n) { g_wp_stats[which] += n; }
+extern "C" int b2h264_dec_wp_stats(long long* out, int n, int reset) {
+  for (int i = 0; i < WPS_N; i++) {
+    if (out && i < n) out[i] = g_wp_stats[i];
+    if (reset) g_wp_stats[i] = 0;
+  }
+  return WPS_N;
+}
+#endif

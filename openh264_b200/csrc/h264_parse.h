@@ -21,7 +21,7 @@ enum ParseError {
   PARSE_OK = 0,
   PARSE_NO_PICTURE = 1,        // the access unit was parsed (parameter sets taken) but holds no slice
   PARSE_TRUNCATED = -1,        // ran out of bits
-  PARSE_UNSUPPORTED = -2,      // valid H.264 outside the supported class (FMO, 8x8 transform, explicit weights, interlace, ...)
+  PARSE_UNSUPPORTED = -2,      // valid H.264 outside the supported class (FMO, scaling lists, interlace, ...)
   PARSE_INVALID = -3,          // not valid H.264 syntax / values out of range
   PARSE_NO_PARAMETER_SETS = -4,// a slice before its SPS / PPS
   PARSE_INCOMPLETE = -5        // the slices seen so far do not cover the picture (more slices of the access unit to come, or lost)

@@ -9,6 +9,7 @@
 #include "mbk_me.cuh"
 #include "mbk_pix8.cuh"
 #include "mbk_sad.cuh"
+#include "wp_formula.h"
 
 using namespace mbk;
 
@@ -181,9 +182,9 @@ __global__ void __launch_bounds__(256) k_weighted_pred(int mode, uint8_t* __rest
     const int y = i / w, x = i - y * w;
     const int p = d[y * stride + x];
     int v;
-    if (mode == 0) v = jb.log2_denom >= 1 ? ((p * jb.w1 + (1 << (jb.log2_denom - 1))) >> jb.log2_denom) + jb.o1 : p * jb.w1 + jb.o1;
-    else if (mode == 1) v = ((p * jb.w1 + t[y * stride + x] * jb.w2 + (1 << jb.log2_denom)) >> (jb.log2_denom + 1)) + ((jb.o1 + jb.o2 + 1) >> 1);
-    else v = (p + t[y * stride + x] + 1) >> 1;
+    if (mode == 0) v = wp_single(p, jb.w1, jb.o1, jb.log2_denom);
+    else if (mode == 1) v = wp_bi(p, t[y * stride + x], jb.w1, jb.w2, wp_bi_offset(jb.o1, jb.o2), jb.log2_denom);
+    else v = wp_bi(p, t[y * stride + x], 1, 1, 0, 0);                   // the plain average (p + q + 1) >> 1
     d[y * stride + x] = (uint8_t)min(max(v, 0), 255);
   }
 }
