@@ -134,6 +134,19 @@ int  b2h264_dec_decode2 (b2h264_dec* d, const uint8_t* const* au, const int32_t*
  * au[s] == NULL), < 0 that stream's own error (-101 .. -105 as above, -2 size mismatch) — it sits the batch out, the other streams are
  * decoded.  The return value only reports errors of the call as a whole (CUDA). */
 int  b2h264_dec_decode3 (b2h264_dec* d, const uint8_t* const* au, const int32_t* au_bytes, uint8_t* const* yuv, int32_t* status);
+/* As b2h264_dec_decode3 (same parsing, same status[s], same error codes), with the pictures left in HBM: yuv_dev[s] is a device
+ * pointer on the decoder's device that receives the cropped, tightly packed I420 picture of stream s (w*h*3/2 bytes, any byte
+ * alignment).  yuv_dev[s] may be NULL only where au[s] is NULL.  A stream that sits the call out or fails keeps its destination
+ * untouched.  Host pointers and pointers on another device are refused with -1 before anything is launched.
+ * ASYNCHRONOUS: the call returns once its work is enqueued on the decoder's stream (b2h264_dec_set_stream); the pictures are
+ * complete when that stream reaches them, so work issued on the same stream afterwards reads finished pictures, and anything else
+ * must wait for the stream.  Each destination must stay allocated until then.  The access units are parsed inside the call and
+ * may be reused on return.  The next call's parse overlaps this call's kernels; the synchronous entry points above may follow a
+ * device call at any time. */
+int  b2h264_dec_decode_device (b2h264_dec* d, const uint8_t* const* au, const int32_t* au_bytes, uint8_t* const* yuv_dev, int32_t* status);
+/* moves all of the decoder's GPU work to the caller's CUDA stream (cudaStream_t as void*), after waiting for the work already
+ * issued on the decoder's current stream (as b2h264_enc_set_stream; the caller keeps the stream alive while the decoder uses it) */
+int  b2h264_dec_set_stream (b2h264_dec* d, void* stream);
 /* Pictures come back in DECODING order.  Of the picture stream `stream` decoded last: its picture order count inside its coded video
  * sequence, *flags (bit 0: an IDR picture — a new sequence starts; bit 1: the picture holds B slices), and the stream's reorder depth (num_ref_frames; 0 for Baseline streams,
  * whose decoding order is the output order).  The reference reorders inside DecodeFrameNoDelay (welsDecoderExt.cpp: ReorderPicturesInDisplay);

@@ -91,6 +91,8 @@ API = {
     "b2h264_dec_decode": [vp, C.POINTER(vp), C.POINTER(C.c_int32), C.POINTER(vp)],
     "b2h264_dec_decode2": [vp, C.POINTER(vp), C.POINTER(C.c_int32), C.POINTER(vp), C.POINTER(C.c_int32)],
     "b2h264_dec_decode3": [vp, C.POINTER(vp), C.POINTER(C.c_int32), C.POINTER(vp), C.POINTER(C.c_int32)],
+    "b2h264_dec_decode_device": [vp, C.POINTER(vp), C.POINTER(C.c_int32), C.POINTER(vp), C.POINTER(C.c_int32)],
+    "b2h264_dec_set_stream": [vp, vp],
     "b2h264_dec_probe": [vp, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)],
     "b2h264_dec_reset_stream": [vp, C.c_int32],
     "b2h264_dec_last_picture_order": [vp, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)],
@@ -293,6 +295,7 @@ class BatchDecoder:
         self.n = n_streams
         self.frame_bytes = width * height * 3 // 2
         self._pin = None
+        self._stream = None            # the CUDA stream handle the decoder was moved to last (b2h264_dec_set_stream)
         if pinned_output:
             self._pin = self.L.b2h264_host_alloc(self.frame_bytes * n_streams)
             if not self._pin:
@@ -335,6 +338,33 @@ class BatchDecoder:
         st = (C.c_int32 * self.n)()
         check(self.L.b2h264_dec_decode3(self.h, au, nb, yo, st))
         return [outs[i] if st[i] == 1 else None for i in range(self.n)], list(st)
+
+    def decode_device(self, access_units, out=None):
+        """like decode3(), with the pictures left on the GPU (b2h264_dec_decode_device): returns (out, status).  out: a
+        (n_streams, w*h*3//2) uint8 CUDA tensor on the decoder's device, allocated when None; row s receives stream s's picture
+        where status[s] == 1 and is left untouched elsewhere.  It may also be a list of n_streams such 1-D tensors (None where the
+        unit is None).  The work runs on torch.cuda.current_stream() and is complete when that stream reaches it."""
+        import torch
+        dev = torch.device("cuda", self.cfg.device)
+        if out is None:
+            out = torch.empty((self.n, self.frame_bytes), dtype=torch.uint8, device=dev)
+        rows = list(out) if isinstance(out, (list, tuple)) else [out[i] for i in range(self.n)] if out.dim() == 2 else None
+        if rows is None or len(rows) != self.n:
+            raise ValueError("out must hold n_streams pictures")
+        for r in rows:
+            if r is not None and (r.dtype != torch.uint8 or r.device != dev or r.numel() != self.frame_bytes or (r.numel() > 1 and r.stride(0) != 1)):
+                raise ValueError("each picture of out must be %d contiguous uint8 bytes on %s" % (self.frame_bytes, dev))
+        st = torch.cuda.current_stream(dev).cuda_stream
+        if st != self._stream:
+            check(self.L.b2h264_dec_set_stream(self.h, st))
+            self._stream = st
+        bufs = [None if a is None else np.frombuffer(bytes(a), np.uint8) for a in access_units]
+        au = (vp * self.n)(*[None if b is None else b.ctypes.data for b in bufs])
+        nb = (C.c_int32 * self.n)(*[0 if b is None else len(b) for b in bufs])
+        yo = (vp * self.n)(*[None if r is None else r.data_ptr() for r in rows])
+        status = (C.c_int32 * self.n)()
+        check(self.L.b2h264_dec_decode_device(self.h, au, nb, yo, status))
+        return out, list(status)
 
     def reset_stream(self, stream):
         check(self.L.b2h264_dec_reset_stream(self.h, stream))

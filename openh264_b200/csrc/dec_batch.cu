@@ -6,13 +6,16 @@
 // WelsTargetMbConstruction (codec/decoder/core/src/decoder_core.cpp, decode_slice.cpp:~100) and
 // WelsDeblockingFilterSlice (deblocking.cpp).  Streams outside the class are rejected with the parser's error
 // code; there is no CPU reconstruction path in this library.
-// Synchronous per call (parse -> H2D -> kernels -> D2H); streams without a slice in their access unit sit the call out.
+// Host output: synchronous per call (parse -> H2D -> kernels -> D2H).  Device output (b2h264_dec_decode_device): the call
+// returns once its work is enqueued, and k_dec_output crops the pictures into the caller's HBM.  Streams without a slice in
+// their access unit sit the call out.
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include <chrono>
+#include <type_traits>
 
 #include <vector>
 
@@ -26,6 +29,11 @@
 using namespace b2h264;
 
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return (int)e_; } while (0)
+
+struct DecOutPic {                        // b2h264_dec_decode_device: one active stream's output
+  const uint8_t* src[3];                  // first sample of each plane inside the crop window of the picture's DPB slot
+  uint8_t* dst;                           // the caller's I420 picture (w*h*3/2 bytes, any alignment)
+};
 
 struct b2h264_dec {
   b2h264_dec_config cfg;
@@ -41,6 +49,8 @@ struct b2h264_dec {
   std::vector<int> act;
   std::vector<uint8_t> act_ref;           // is the picture of act[i] a reference picture
   cudaStream_t st = nullptr;
+  bool own_stream = true;                 // false after b2h264_dec_set_stream: the caller's stream is not destroyed here
+  cudaEvent_t staged = nullptr;           // after the last host-to-device copy of a call: the pinned buffers may be rewritten
   uint8_t* d_pic = nullptr;               // S x slots padded pictures: picture (s, slot) at (s * slots + slot) * pic_bytes
   MbInfo* d_mbi = nullptr;
   MbOut* d_recs = nullptr;
@@ -56,6 +66,8 @@ struct b2h264_dec {
   std::vector<int> last_poc, last_idr, last_reorder;   // per stream: picture order count / IDR flag / reorder depth of the last decoded picture
   StreamFrame* d_sf = nullptr;
   StreamFrame* h_sf = nullptr;            // pinned
+  DecOutPic* d_out = nullptr;             // device output: per active stream, the sources and the destination of its planes
+  DecOutPic* h_out = nullptr;             // pinned
   int* d_ws = nullptr;
   size_t pic_bytes = 0, pic_y_bytes = 0, pic_c_bytes = 0;
   int last_error_stream = -1;
@@ -67,6 +79,41 @@ struct b2h264_dec {
     return base + pic_y_bytes + (size_t)(pl - 1) * pic_c_bytes + (size_t)16 * stc + 16;
   }
 };
+
+// ---- device output: the cropped pictures of one call into the caller's HBM, every active stream and plane in one launch ----
+// One warp per row of a plane.  A row is copied in the widest words (16, 8, 4 or 1 bytes) that its source and destination
+// share an alignment for: the destination's head bytes go one by one, then whole words, then the tail.
+template <int V>
+__device__ __forceinline__ void out_row(const uint8_t* src, uint8_t* dst, int n, int lane) {
+  int head = (int)((0u - (unsigned)(uintptr_t)dst) & (V - 1));
+  if (head > n) head = n;
+  if (lane < head) dst[lane] = src[lane];
+  const int words = (n - head) / V;
+  // word-aligned because source and destination agree modulo V; rounding the source down only makes that explicit
+  typedef typename std::conditional<V == 16, uint4, typename std::conditional<V == 8, uint2, uint32_t>::type>::type W;
+  const W* s = reinterpret_cast<const W*>((uintptr_t)(src + head) & ~(uintptr_t)(V - 1));
+  W* d = reinterpret_cast<W*>(dst + head);
+  for (int k = lane; k < words; k += 32) d[k] = __ldg(s + k);
+  const int t = head + words * V + lane;
+  if (t < n) dst[t] = src[t];
+}
+
+__global__ void __launch_bounds__(256) k_dec_output(const DecOutPic* __restrict__ pics, int w, int h, int sty, int stc) {
+  const int lane = threadIdx.x & 31;
+  const int r = blockIdx.x * 8 + (threadIdx.x >> 5);   // row over the three planes: h luma rows, then h / 2 of each chroma plane
+  if (r >= 2 * h) return;
+  const DecOutPic& P = pics[blockIdx.y];
+  const int pl = r < h ? 0 : r < h + h / 2 ? 1 : 2;
+  const int y = pl == 0 ? r : r - h - (pl - 1) * (h / 2);
+  const int n = pl ? w / 2 : w;
+  const uint8_t* src = P.src[pl] + (size_t)y * (pl ? stc : sty);
+  uint8_t* dst = P.dst + (pl ? (size_t)w * h + (size_t)(pl - 1) * (w / 2) * (h / 2) : 0) + (size_t)y * n;
+  const unsigned mis = (unsigned)(((uintptr_t)src ^ (uintptr_t)dst) & 15);
+  if (mis == 0) out_row<16>(src, dst, n, lane);
+  else if ((mis & 7) == 0) out_row<8>(src, dst, n, lane);
+  else if ((mis & 3) == 0) out_row<4>(src, dst, n, lane);
+  else for (int x = lane; x < n; x += 32) dst[x] = src[x];
+}
 
 extern "C" {
 
@@ -105,6 +152,9 @@ int b2h264_dec_create(const b2h264_dec_config* cfg, b2h264_dec** out) {
   CK(cudaMallocHost(&d->h_aux, S * d->n_mb * sizeof(DecMbAux)));
   CK(cudaMalloc(&d->d_sf, S * sizeof(StreamFrame)));
   CK(cudaMallocHost(&d->h_sf, S * sizeof(StreamFrame)));
+  CK(cudaMalloc(&d->d_out, S * sizeof(DecOutPic)));
+  CK(cudaMallocHost(&d->h_out, S * sizeof(DecOutPic)));
+  CK(cudaEventCreateWithFlags(&d->staged, cudaEventDisableTiming));
   CK(cudaMalloc(&d->d_ws, dec_sched_ints((int)S, d->mb_w, d->mb_h) * sizeof(int)));
   *out = d;
   return 0;
@@ -119,7 +169,9 @@ void b2h264_dec_destroy(b2h264_dec* d) {
   if (d->d_aux_b) cudaFree(d->d_aux_b);
   if (d->h_aux_b) cudaFreeHost(d->h_aux_b);
   cudaFreeHost(d->h_recs); cudaFreeHost(d->h_sf); cudaFree(d->d_pack); cudaFreeHost(d->h_idx); cudaFree(d->d_idx);
-  if (d->st) cudaStreamDestroy(d->st);
+  cudaFree(d->d_out); cudaFreeHost(d->h_out);
+  if (d->staged) cudaEventDestroy(d->staged);
+  if (d->st && d->own_stream) cudaStreamDestroy(d->st);
   delete d->pool;
   delete d;
 }
@@ -129,7 +181,9 @@ void b2h264_dec_destroy(b2h264_dec* d) {
 // status (may be NULL): per-stream outcome for callers that batch UNRELATED streams (the ISVCDecoder broker): 1 = picture, 0 = no slice in
 // the unit, < 0 = this stream's error (-101 .. -105, -2) — such a stream sits the batch out and the others are decoded; without
 // `status` the first stream error ends the call (the streams of one application stand or fall together).
-static int dec_decode_impl(b2h264_dec* d, const uint8_t* const* au, const int32_t* au_bytes, uint8_t* const* yuv, int32_t* got_picture, int32_t* status) {
+// on_device: yuv[s] are device pointers on the decoder's device, written by k_dec_output; the call returns once its work is enqueued.
+static int dec_decode_impl(b2h264_dec* d, const uint8_t* const* au, const int32_t* au_bytes, uint8_t* const* yuv, int32_t* got_picture, int32_t* status,
+                           bool on_device = false) {
   if (!d || !au || !au_bytes || !yuv) return -1;
   CK(cudaSetDevice(d->cfg.device));
   const int S = d->S;
@@ -153,6 +207,8 @@ static int dec_decode_impl(b2h264_dec* d, const uint8_t* const* au, const int32_
     d->pool->run(S, job);
   }
   const double t_parse = ms_since(t0);
+  // the pinned staging buffers still feed the previous call's copies until they are issued: the parse above overlapped them
+  CK(cudaEventSynchronize(d->staged));
   // 2. the batch: descriptors and records of the streams that carry a picture, in stream order
 #define STREAM_FAIL(code) { d->last_error_stream = s; if (status) { status[s] = (code); continue; } return (code); }
   if (status) for (int s = 0; s < S; s++) status[s] = 0;
@@ -233,6 +289,19 @@ static int dec_decode_impl(b2h264_dec* d, const uint8_t* const* au, const int32_
     if (d->parsed[d->act[i]].has_b)
       CK(cudaMemcpyAsync(d->d_aux_b + (size_t)i * d->n_mb, d->h_aux_b + (size_t)i * d->n_mb, (size_t)d->n_mb * sizeof(DecMbAuxB), cudaMemcpyHostToDevice, d->st));
   CK(cudaMemcpyAsync(d->d_sf, d->h_sf, (size_t)n * sizeof(StreamFrame), cudaMemcpyHostToDevice, d->st));
+  const int w = d->cfg.width, h = d->cfg.height;
+  if (on_device) {
+    for (int i = 0; i < n; i++) {
+      DecOutPic& O = d->h_out[i];
+      for (int pl = 0; pl < 3; pl++) {
+        const int c = pl ? 1 : 0;
+        O.src[pl] = d->plane0(d->out_slot[i], d->act[i], pl) + (size_t)(d->out_cy[i] >> c) * (pl ? d->geo.rec_stride_c() : d->geo.rec_stride_y()) + (d->out_cx[i] >> c);
+      }
+      O.dst = yuv[d->act[i]];
+    }
+    CK(cudaMemcpyAsync(d->d_out, d->h_out, (size_t)n * sizeof(DecOutPic), cudaMemcpyHostToDevice, d->st));
+  }
+  CK(cudaEventRecord(d->staged, d->st));
   int b_slices = 0;
   for (int i = 0; i < n; i++) b_slices |= (d->parsed[d->act[i]].has_b || d->parsed[d->act[i]].has_t8) ? 1 : 0;   // Main / High tools: the wider filter kernel
   const int rc = dec_launch_frame(d->d_sf, n, d->mb_w, d->mb_h, d->d_ws, d->d_recs, d->d_aux, deblock, d->st, b_slices);
@@ -240,7 +309,13 @@ static int dec_decode_impl(b2h264_dec* d, const uint8_t* const* au, const int32_
   const double t_launch = ms_since(t0);
   if (timing) cudaStreamSynchronize(d->st);
   const double t_kernels = ms_since(t0);
-  const int w = d->cfg.width, h = d->cfg.height;
+  if (on_device) {
+    k_dec_output<<<dim3((2 * h + 7) / 8, n), 256, 0, d->st>>>(d->d_out, w, h, d->geo.rec_stride_y(), d->geo.rec_stride_c());
+    const int rco = b2h264_launched();
+    if (rco) return rco;
+    for (int i = 0; i < n; i++) status[d->act[i]] = 1;
+    return 0;
+  }
   for (int i = 0; i < n; i++) {
     const int s = d->act[i], rec = d->out_slot[i];
     uint8_t* dst = yuv[s];
@@ -275,6 +350,29 @@ int b2h264_dec_decode3(b2h264_dec* d, const uint8_t* const* au, const int32_t* a
 }
 int b2h264_dec_decode(b2h264_dec* d, const uint8_t* const* au, const int32_t* au_bytes, uint8_t* const* yuv) {
   return dec_decode_impl(d, au, au_bytes, yuv, nullptr, nullptr);
+}
+int b2h264_dec_decode_device(b2h264_dec* d, const uint8_t* const* au, const int32_t* au_bytes, uint8_t* const* yuv_dev, int32_t* status) {
+  if (!d || !au || !au_bytes || !yuv_dev || !status) return -1;
+  CK(cudaSetDevice(d->cfg.device));
+  for (int s = 0; s < d->S; s++) {                       // every destination that may be written: HBM of the decoder's device
+    if (!au[s]) continue;
+    cudaPointerAttributes at;
+    if (!yuv_dev[s] || cudaPointerGetAttributes(&at, yuv_dev[s]) != cudaSuccess || at.type != cudaMemoryTypeDevice || at.device != d->cfg.device) {
+      (void)cudaGetLastError();
+      return -1;
+    }
+  }
+  return dec_decode_impl(d, au, au_bytes, yuv_dev, nullptr, status, true);
+}
+
+int b2h264_dec_set_stream(b2h264_dec* d, void* stream) {
+  if (!d) return -1;
+  CK(cudaSetDevice(d->cfg.device));
+  CK(cudaStreamSynchronize(d->st));
+  if (d->own_stream) CK(cudaStreamDestroy(d->st));
+  d->st = (cudaStream_t)stream;
+  d->own_stream = false;
+  return 0;
 }
 
 // Looks at an access unit without a decoder: *has_slice = a coded slice NAL is present; if it carries an SPS of the
