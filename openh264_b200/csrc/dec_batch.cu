@@ -195,14 +195,7 @@ static int dec_decode_impl(b2h264_dec* d, const uint8_t* const* au, const int32_
   // 1. parse: every stream's access unit on the pool (streams are independent; a stream's parser state is its own)
   {
     std::function<void(int)> job = [&](int s) {
-      ParsedPicture& pp = d->parsed[s];               // a fresh picture that keeps the record arrays' storage
-      std::vector<MbOut> m = std::move(pp.mbs);
-      std::vector<DecMbAux> a = std::move(pp.aux);
-      std::vector<DecMbAuxB> ab = std::move(pp.aux_b);
-      std::vector<CabacMbInfo> ci = std::move(pp.cabac_info);
-      pp = ParsedPicture();
-      pp.mbs = std::move(m); pp.aux = std::move(a); pp.aux_b = std::move(ab); pp.cabac_info = std::move(ci);
-      d->parse_rc[s] = (!au[s] || au_bytes[s] <= 0) ? PARSE_NO_PICTURE : parse_access_unit(au[s], (size_t)au_bytes[s], &d->parser[s], &pp);
+      d->parse_rc[s] = (!au[s] || au_bytes[s] <= 0) ? PARSE_NO_PICTURE : parse_access_unit(au[s], (size_t)au_bytes[s], &d->parser[s], &d->parsed[s]);
     };
     d->pool->run(S, job);
   }

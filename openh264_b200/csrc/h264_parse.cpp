@@ -7,6 +7,8 @@
 #include <stddef.h>
 #include <string.h>
 
+#include <algorithm>
+
 
 #include "cavlc_tables.h"
 #include "h264_cabac_dec.h"
@@ -380,750 +382,698 @@ int cbp_from_code(int code, bool intra) {
   return inv[intra ? 1 : 0][code];
 }
 
-int parse_slice(BitReader& r, const Nal& nal, ParserState* st, ParsedPicture* pic) {
-  const bool idr = nal.type == 5;
-  if (!idr && !st->have_ref) return PARSE_INVALID;            // a P picture before any IDR: nothing to predict from
+// One slice: what its header says (7.3.3), and the state its macroblocks are parsed with.
+struct SliceCtx {
+  ParserState* st = nullptr;
+  ParsedPicture* pic = nullptr;
+  bool idr = false, is_ref = false, is_p = false, is_b = false, inter = false;
+  int first_mb = 0;
+  SliceState ss{};               // idr, frame_num, idr_pic_id, slice QP
+  int poc = 0, poc_msb = 0, poc_lsb = 0;
+  int n_ref[2] = {0, 0};         // num_ref_idx_l0_active, num_ref_idx_l1_active
+  RefEntry lists[2][33];         // RefPicList0 / RefPicList1; entries carry the picture SLOT of the construct stage
+  WpTable wp;                    // pred_weight_table
+  bool adaptive_marking = false, idr_long_term = false;
+  std::vector<ParsedPicture::Mmco> mmco;
+  int cabac_init_idc = 0;
+  int dbk_idc = 0, alpha_off = 0, beta_off = 0;   // disable_deblocking_filter_idc, FilterOffsetA / B
+  int slice_no = 0, mbw = 0, n_mb = 0;
+  // host-side motion derivation (h264_motion.h): the field of every picture where B slices may occur, B macroblocks resolved here
+  bool track = false;
+  bool track_fail = false;       // a P macroblock with explicit weights could not be resolved
+  MotionCtx M;
+  BSliceCtx b;                   // B slices: direct prediction, lists and weights as motion resolution reads them
+};
+
+// a picture of the buffer as a list entry; identity PicNum (FrameNumWrap, 8.2.4.1), or LongTermPicNum (= LongTermFrameIdx) + 2^20
+RefEntry ref_entry(const ParserState::RefPic& rp, int frame_num, int max_fn) {
+  RefEntry e;
+  e.slot = rp.slot; e.poc = rp.poc; e.pic_id = rp.pic_id; e.lt = rp.long_term;
+  e.key = rp.long_term ? rp.lt_idx + (1 << 20) : (rp.frame_num > frame_num ? rp.frame_num - max_fn : rp.frame_num);
+  return e;
+}
+
+// initial RefPicList0 / RefPicList1 (8.2.4.2): P slices order the short-term pictures by descending PicNum, B slices by picture
+// order count around the current picture; long-term pictures follow by ascending LongTermPicNum
+int init_ref_lists(const ParserState* st, SliceCtx& c) {
+  RefEntry cand[32];
+  int nc = 0;
+  for (const ParserState::RefPic& rp : st->refs) {
+    if (nc >= 32) break;
+    cand[nc++] = ref_entry(rp, c.ss.frame_num, 1 << st->log2_max_frame_num);
+  }
+  if (nc == 0) return PARSE_INVALID;
+  int no[2] = {0, 0};
+  auto append_sorted = [&](int l, auto pick, auto before) {   // the candidates `pick` selects, in a stable order by `before`
+    const int first = no[l];
+    for (int i = 0; i < nc; i++) if (pick(cand[i])) c.lists[l][no[l]++] = cand[i];
+    std::stable_sort(c.lists[l] + first, c.lists[l] + no[l], before);
+  };
+  auto is_lt = [](const RefEntry& e) { return e.lt; };
+  auto key_asc = [](const RefEntry& a, const RefEntry& b) { return a.key < b.key; };
+  if (c.is_p) {
+    append_sorted(0, [](const RefEntry& e) { return !e.lt; }, [](const RefEntry& a, const RefEntry& b) { return a.key > b.key; });
+    append_sorted(0, is_lt, key_asc);
+  } else {
+    const int poc = c.poc;
+    auto poc_desc = [](const RefEntry& a, const RefEntry& b) { return a.poc > b.poc; };
+    auto poc_asc = [](const RefEntry& a, const RefEntry& b) { return a.poc < b.poc; };
+    auto before_cur = [poc](const RefEntry& e) { return !e.lt && e.poc < poc; };
+    auto after_cur = [poc](const RefEntry& e) { return !e.lt && e.poc > poc; };
+    append_sorted(0, before_cur, poc_desc); append_sorted(0, after_cur, poc_asc); append_sorted(0, is_lt, key_asc);
+    append_sorted(1, after_cur, poc_asc); append_sorted(1, before_cur, poc_desc); append_sorted(1, is_lt, key_asc);
+    auto same_pic = [](const RefEntry& a, const RefEntry& b) { return a.pic_id == b.pic_id && a.slot == b.slot; };
+    if (no[1] > 1 && no[0] == no[1] && std::equal(c.lists[0], c.lists[0] + no[0], c.lists[1], same_pic))
+      std::swap(c.lists[1][0], c.lists[1][1]);                // identical lists: the first two entries of list 1 change places
+  }
+  for (int l = 0; l < (c.is_b ? 2 : 1); l++)
+    for (int i = no[l]; i < 33; i++) {
+      if (c.is_p && no[l] > 0) { c.lists[l][i] = c.lists[l][no[l] - 1]; c.lists[l][i].key = -0x40000000; }   // entries past the
+      else c.lists[l][i] = RefEntry();                                           // available pictures (a conforming stream does not use them)
+    }
+  return PARSE_OK;
+}
+
+// ref_pic_list_modification() of list l (7.3.3.1), each command applied as it is read (8.2.4.3)
+int modify_ref_list(BitReader& r, const ParserState* st, SliceCtx& c, int l) {
+  if (!r.bit()) return PARSE_OK;                              // ref_pic_list_modification_flag_lX
+  const int max_fn = 1 << st->log2_max_frame_num, nref_l = c.n_ref[l];
+  RefEntry* L = c.lists[l];
+  int pred = c.ss.frame_num, idx = 0;
+  for (;;) {
+    const uint32_t idc = r.ue();
+    if (idc == 3) return PARSE_OK;
+    if (idc > 3 || !r.ok()) return PARSE_INVALID;
+    const uint32_t v = r.ue();
+    if (idx >= nref_l) return PARSE_INVALID;
+    int want;
+    if (idc == 2) {
+      want = (int)v + (1 << 20);                              // long_term_pic_num
+    } else {
+      if (v >= (uint32_t)max_fn) return PARSE_INVALID;
+      int no_wrap = idc == 0 ? pred - ((int)v + 1) : pred + ((int)v + 1);
+      if (no_wrap < 0) no_wrap += max_fn;
+      if (no_wrap >= max_fn) no_wrap -= max_fn;
+      pred = no_wrap;
+      want = no_wrap > c.ss.frame_num ? no_wrap - max_fn : no_wrap;
+    }
+    bool found = false;                                       // the last of the (first 32) pictures of the buffer with that identity
+    RefEntry e;
+    for (size_t i = 0; i < st->refs.size() && i < 32; i++) {
+      const RefEntry x = ref_entry(st->refs[i], c.ss.frame_num, max_fn);
+      if (x.key == want) { e = x; found = true; }
+    }
+    if (!found) return PARSE_UNSUPPORTED;                     // refers to a picture that is not in the buffer (loss): needs concealment
+    // insert at idx, shift the rest, drop the later duplicate
+    for (int k = nref_l; k > idx; k--) L[k] = L[k - 1];
+    L[idx++] = e;
+    int nidx = idx;
+    for (int k = idx; k <= nref_l; k++)
+      if (L[k].key != want) L[nidx++] = L[k];
+  }
+}
+
+// pred_weight_table() (7.3.3.2)
+int read_pred_weight_table(BitReader& r, const ParserState* st, SliceCtx& c) {
+  WpTable& wp = c.wp;
+  wp.on = true;
+  const uint32_t dl = r.ue(), dc = r.ue();
+  if (dl > 7 || dc > 7) return PARSE_INVALID;
+  wp.log2[0] = (int)dl; wp.log2[1] = (int)dc;
+  for (int l = 0; l < (c.is_b ? 2 : 1); l++)
+    for (int i = 0; i < c.n_ref[l]; i++) {
+      int given = 0;                                          // luma_weight_flag (bit 0), chroma_weight_flag (bit 1)
+      for (int pl = 0; pl < 3; pl++) {
+        if (pl < 2) given |= r.bit() << pl;
+        int w = 1 << wp.log2[pl ? 1 : 0], o = 0;              // absent: the default weight and offset
+        if ((given >> (pl ? 1 : 0)) & 1) {
+          w = r.se(); o = r.se();
+          if (w < -128 || w > 127 || o < -128 || o > 127) return PARSE_INVALID;
+        }
+        wp.w[l][i][pl][0] = (int16_t)w; wp.w[l][i][pl][1] = (int16_t)o;
+      }
+      wp.given[l][i] = (uint8_t)given;
+    }
+  if (!r.ok()) return PARSE_TRUNCATED;
+  if (st->profile == 66) return PARSE_INVALID;
+  return PARSE_OK;
+}
+
+// dec_ref_pic_marking() (7.3.3.3) of a reference picture's slice
+int read_dec_ref_pic_marking(BitReader& r, SliceCtx& c) {
+  if (c.idr) { r.bit(); c.idr_long_term = r.bit() != 0; return PARSE_OK; }   // no_output_of_prior_pics_flag, long_term_reference_flag
+  if (!r.bit()) return PARSE_OK;                              // adaptive_ref_pic_marking_mode_flag 0: sliding window
+  c.adaptive_marking = true;
+  for (;;) {
+    ParsedPicture::Mmco m;
+    m.op = (int)r.ue(); m.a = m.b = 0;
+    if (m.op == 0) return PARSE_OK;
+    if (m.op > 6 || !r.ok()) return PARSE_INVALID;
+    if (m.op == 1 || m.op == 3) m.a = (int)r.ue();            // difference_of_pic_nums_minus1
+    if (m.op == 2) m.a = (int)r.ue();                         // long_term_pic_num
+    if (m.op == 3 || m.op == 6) m.b = (int)r.ue();            // long_term_frame_idx
+    if (m.op == 4) m.a = (int)r.ue();                         // max_long_term_frame_idx_plus1
+    c.mmco.push_back(m);
+    if (c.mmco.size() > 64) return PARSE_INVALID;
+  }
+}
+
+// slice_header() (7.3.3): activates the slice's parameter sets and builds its reference lists (8.2.4)
+int parse_slice_header(BitReader& r, const Nal& nal, ParserState* st, const ParsedPicture* pic, SliceCtx& c) {
+  c.idr = nal.type == 5;
+  if (!c.idr && !st->have_ref) return PARSE_INVALID;          // a P picture before any IDR: nothing to predict from
   const bool first_slice = pic->n_slices == 0;
-  const int first_mb = (int)r.ue();
-  if (first_mb != pic->next_mb) return PARSE_UNSUPPORTED;     // slices out of raster order / missing slices (ASO, FMO, losses)
+  c.first_mb = (int)r.ue();
+  if (c.first_mb != pic->next_mb) return PARSE_UNSUPPORTED;   // slices out of raster order / missing slices (ASO, FMO, losses)
   const int slice_type = (int)r.ue() % 5;
   if (slice_type > 2) return PARSE_UNSUPPORTED;               // SP / SI slices
-  const bool is_p = slice_type == 0, is_b = slice_type == 1, inter_slice = is_p || is_b;
-  if (idr && inter_slice) return PARSE_INVALID;
+  c.is_p = slice_type == 0; c.is_b = slice_type == 1; c.inter = c.is_p || c.is_b;
+  if (c.idr && c.inter) return PARSE_INVALID;
   {                                                           // the slice names its PPS, the PPS its SPS (several of each may be around)
     const uint32_t id = r.ue();
     if (id > 255 || !st->pps_tab[id].valid || !st->sps_tab[st->pps_tab[id].sps_id].valid) return PARSE_NO_PARAMETER_SETS;
     if (!first_slice && (int)id != st->sp.pps_id && st->pps_tab[id].sps_id != st->sp.sps_id) return PARSE_INVALID;
     if (first_slice && (st->sp.sps_id != st->pps_tab[id].sps_id || !st->have_sps)) {
-      if (!idr && st->have_sps) return PARSE_UNSUPPORTED;     // a new sequence may only start at an IDR picture
+      if (!c.idr && st->have_sps) return PARSE_UNSUPPORTED;   // a new sequence may only start at an IDR picture
       activate_sps(st, st->pps_tab[id].sps_id);
     }
     activate_pps(st, (int)id);
   }
   // B slices: where the profile has them, with picture order count type 0 and direct_8x8_inference (frame macroblocks: the corner
   // blocks of the co-located macroblock stand for its 8x8 blocks)
-  if (is_b && (st->profile == 66 || st->poc_type != 0 || !st->direct_8x8_inference)) return PARSE_UNSUPPORTED;
-  const int mbw = st->sp.mb_w, n = st->sp.mb_w * st->sp.mb_h;
-  SliceState ss;
-  ss.idr = idr;
-  ss.frame_num = (int)r.get(st->log2_max_frame_num);
-  ss.idr_pic_id = idr ? (int)r.ue() : 0;
-  int poc_lsb = 0, poc_msb = 0, poc;
-  if (st->poc_type == 0) poc_lsb = (int)r.get(st->log2_max_poc_lsb);
+  if (c.is_b && (st->profile == 66 || st->poc_type != 0 || !st->direct_8x8_inference)) return PARSE_UNSUPPORTED;
+  c.ss.idr = c.idr;
+  c.ss.frame_num = (int)r.get(st->log2_max_frame_num);
+  c.ss.idr_pic_id = c.idr ? (int)r.ue() : 0;
+  if (st->poc_type == 0) c.poc_lsb = (int)r.get(st->log2_max_poc_lsb);
   else if (st->poc_type == 1 && !st->delta_pic_order_always_zero) r.se();          // delta_pic_order_cnt[0]
   if (st->poc_type == 0) {                                    // 8.2.1.1
     const int max_lsb = 1 << st->log2_max_poc_lsb;
-    const int prev_msb = idr ? 0 : st->prev_poc_msb, prev_lsb = idr ? 0 : st->prev_poc_lsb;
-    if (poc_lsb < prev_lsb && prev_lsb - poc_lsb >= max_lsb / 2) poc_msb = prev_msb + max_lsb;
-    else if (poc_lsb > prev_lsb && poc_lsb - prev_lsb > max_lsb / 2) poc_msb = prev_msb - max_lsb;
-    else poc_msb = prev_msb;
-    poc = poc_msb + poc_lsb;
+    const int prev_msb = c.idr ? 0 : st->prev_poc_msb, prev_lsb = c.idr ? 0 : st->prev_poc_lsb;
+    if (c.poc_lsb < prev_lsb && prev_lsb - c.poc_lsb >= max_lsb / 2) c.poc_msb = prev_msb + max_lsb;
+    else if (c.poc_lsb > prev_lsb && c.poc_lsb - prev_lsb > max_lsb / 2) c.poc_msb = prev_msb - max_lsb;
+    else c.poc_msb = prev_msb;
+    c.poc = c.poc_msb + c.poc_lsb;
   } else {
-    poc = 2 * (idr ? 0 : st->decode_count);                   // types 1 / 2 without B slices: output order is decoding order
+    c.poc = 2 * (c.idr ? 0 : st->decode_count);               // types 1 / 2 without B slices: output order is decoding order
   }
-  const bool direct_spatial = is_b ? r.bit() != 0 : true;     // direct_spatial_mv_pred_flag
-  // RefPicList0 / RefPicList1 of this slice (8.2.4.2): P slices order the short-term pictures by descending PicNum, B slices by
-  // picture order count around the current picture; long-term pictures follow by ascending LongTermPicNum; then the slice's
-  // modification commands (8.2.4.3).  Entries carry the picture SLOT of the construct stage.
-  RefEntry lists[2][33];
-  int list0[32];
-  int n_ref = 0, n_ref1 = 0;
-  if (inter_slice) {
-    n_ref = st->num_ref_idx_default;
-    n_ref1 = is_b ? st->num_ref_idx_l1_default : 0;
-    if (r.bit()) { n_ref = (int)r.ue() + 1; if (is_b) n_ref1 = (int)r.ue() + 1; }
-    if (n_ref < 1 || n_ref > 32 || (is_b && (n_ref1 < 1 || n_ref1 > 32))) return PARSE_INVALID;
-    const int max_fn = 1 << st->log2_max_frame_num;
-    // key: short-term pictures by PicNum (FrameNumWrap), long-term pictures by LongTermPicNum (= LongTermFrameIdx for frames)
-    struct Cand { int slot, num; bool lt; int poc, pic_id; };
-    Cand cand[32];
-    int nc = 0;
-    for (const ParserState::RefPic& rp : st->refs) {
-      if (nc >= 32) break;
-      cand[nc].slot = rp.slot; cand[nc].lt = rp.long_term; cand[nc].poc = rp.poc; cand[nc].pic_id = rp.pic_id;
-      cand[nc].num = rp.long_term ? rp.lt_idx : (rp.frame_num > ss.frame_num ? rp.frame_num - max_fn : rp.frame_num);      // FrameNumWrap
-      nc++;
-    }
-    if (nc == 0) return PARSE_INVALID;
-    auto key_of = [](const Cand& c) { return c.lt ? c.num + (1 << 20) : c.num; };   // identity of an entry: PicNum, or LongTermPicNum + 2^20
-    auto entry_of = [&](const Cand& c) { RefEntry e; e.slot = c.slot; e.key = key_of(c); e.poc = c.poc; e.pic_id = c.pic_id; e.lt = c.lt; return e; };
-    int ord[2][32], no[2] = {0, 0};
-    auto append_sorted = [&](int l, auto pick, auto before) {   // the candidates `pick` selects, ordered by `before`
-      const int first = no[l];
-      for (int i = 0; i < nc; i++) {
-        if (!pick(cand[i])) continue;
-        int j = no[l]++;
-        ord[l][j] = i;
-        for (; j > first && before(cand[ord[l][j]], cand[ord[l][j - 1]]); j--) { const int t = ord[l][j]; ord[l][j] = ord[l][j - 1]; ord[l][j - 1] = t; }
-      }
-    };
-    auto lt_asc = [](const Cand& a, const Cand& b) { return a.num < b.num; };
-    auto is_lt = [](const Cand& c) { return c.lt; };
-    if (is_p) {
-      append_sorted(0, [](const Cand& c) { return !c.lt; }, [](const Cand& a, const Cand& b) { return a.num > b.num; });
-      append_sorted(0, is_lt, lt_asc);
-    } else {
-      auto poc_desc = [](const Cand& a, const Cand& b) { return a.poc > b.poc; };
-      auto poc_asc = [](const Cand& a, const Cand& b) { return a.poc < b.poc; };
-      auto before_cur = [&](const Cand& c) { return !c.lt && c.poc < poc; };
-      auto after_cur = [&](const Cand& c) { return !c.lt && c.poc > poc; };
-      append_sorted(0, before_cur, poc_desc); append_sorted(0, after_cur, poc_asc); append_sorted(0, is_lt, lt_asc);
-      append_sorted(1, after_cur, poc_asc); append_sorted(1, before_cur, poc_desc); append_sorted(1, is_lt, lt_asc);
-      if (no[1] > 1 && no[0] == no[1]) {                      // identical lists: the first two entries of list 1 change places
-        bool same = true;
-        for (int i = 0; i < no[0]; i++) same = same && ord[0][i] == ord[1][i];
-        if (same) { const int t = ord[1][0]; ord[1][0] = ord[1][1]; ord[1][1] = t; }
-      }
-    }
-    for (int l = 0; l < (is_b ? 2 : 1); l++)
-      for (int i = 0; i < 33; i++) {
-        if (i < no[l]) lists[l][i] = entry_of(cand[ord[l][i]]);
-        else if (is_p && no[l] > 0) { lists[l][i] = entry_of(cand[ord[l][no[l] - 1]]); lists[l][i].key = -0x40000000; }   // entries past the available
-        else lists[l][i] = RefEntry();                                                            // pictures (a conforming stream does not use them)
-      }
-    for (int l = 0; l < (is_b ? 2 : 1); l++) {
-      const int nref_l = l ? n_ref1 : n_ref;
-      RefEntry* L = lists[l];
-      if (!r.bit()) continue;                                 // ref_pic_list_modification_flag_lX (8.2.4.3)
-      int pred = ss.frame_num, idx = 0;
-      for (;;) {
-        const uint32_t idc = r.ue();
-        if (idc == 3) break;
-        if (idc > 3 || !r.ok()) return PARSE_INVALID;
-        const uint32_t v = r.ue();
-        if (idx >= nref_l) return PARSE_INVALID;
-        int want;
-        if (idc == 2) {
-          want = (int)v + (1 << 20);                          // long_term_pic_num
-        } else {
-          if (v >= (uint32_t)max_fn) return PARSE_INVALID;
-          int no_wrap = idc == 0 ? pred - ((int)v + 1) : pred + ((int)v + 1);
-          if (no_wrap < 0) no_wrap += max_fn;
-          if (no_wrap >= max_fn) no_wrap -= max_fn;
-          pred = no_wrap;
-          want = no_wrap > ss.frame_num ? no_wrap - max_fn : no_wrap;
-        }
-        int found = -1;
-        for (int i = 0; i < nc; i++) if (key_of(cand[i]) == want) found = i;
-        if (found < 0) return PARSE_UNSUPPORTED;              // refers to a picture that is not in the buffer (loss): needs concealment
-        // insert at idx, shift the rest, drop the later duplicate
-        for (int c = nref_l; c > idx; c--) L[c] = L[c - 1];
-        L[idx] = entry_of(cand[found]);
-        idx++;
-        int nidx = idx;
-        for (int c = idx; c <= nref_l; c++)
-          if (L[c].key != want) L[nidx++] = L[c];
-      }
-    }
-    for (int i = 0; i < 32; i++) list0[i] = lists[0][i].slot;
-    for (int i = 0; i < n_ref; i++) if (list0[i] < 0 && is_p) return PARSE_INVALID;
+  if (c.is_b) c.b.direct_spatial = r.bit() != 0;              // direct_spatial_mv_pred_flag
+  int rc;
+  if (c.inter) {
+    c.n_ref[0] = st->num_ref_idx_default;
+    c.n_ref[1] = c.is_b ? st->num_ref_idx_l1_default : 0;
+    if (r.bit()) { c.n_ref[0] = (int)r.ue() + 1; if (c.is_b) c.n_ref[1] = (int)r.ue() + 1; }   // num_ref_idx_active_override_flag
+    if (c.n_ref[0] < 1 || c.n_ref[0] > 32 || (c.is_b && (c.n_ref[1] < 1 || c.n_ref[1] > 32))) return PARSE_INVALID;
+    if ((rc = init_ref_lists(st, c)) != PARSE_OK) return rc;
+    for (int l = 0; l < (c.is_b ? 2 : 1); l++)
+      if ((rc = modify_ref_list(r, st, c, l)) != PARSE_OK) return rc;
+    for (int i = 0; i < c.n_ref[0]; i++) if (c.lists[0][i].slot < 0 && c.is_p) return PARSE_INVALID;
   }
-  // pred_weight_table (7.3.3.2): explicit weights of a P slice (weighted_pred_flag) or a B slice (weighted_bipred_idc 1)
-  WpTable wp;
-  if ((is_p && st->weighted_pred) || (is_b && st->weighted_bipred_idc == 1)) {
-    wp.on = true;
-    const uint32_t dl = r.ue(), dc = r.ue();
-    if (dl > 7 || dc > 7) return PARSE_INVALID;
-    wp.log2[0] = (int)dl; wp.log2[1] = (int)dc;
-    for (int l = 0; l < (is_b ? 2 : 1); l++)
-      for (int i = 0; i < (l ? n_ref1 : n_ref); i++) {
-        for (int pl = 0; pl < 3; pl++) { wp.w[l][i][pl][0] = (int16_t)(1 << wp.log2[pl ? 1 : 0]); wp.w[l][i][pl][1] = 0; }
-        const int luma_flag = r.bit();
-        if (luma_flag) {
-          const int w = r.se(), o = r.se();
-          if (w < -128 || w > 127 || o < -128 || o > 127) return PARSE_INVALID;
-          wp.w[l][i][0][0] = (int16_t)w; wp.w[l][i][0][1] = (int16_t)o;
-        }
-        const int chroma_flag = r.bit();
-        wp.given[l][i] = (uint8_t)(luma_flag | chroma_flag << 1);
-        if (chroma_flag)
-          for (int pl = 1; pl < 3; pl++) {
-            const int w = r.se(), o = r.se();
-            if (w < -128 || w > 127 || o < -128 || o > 127) return PARSE_INVALID;
-            wp.w[l][i][pl][0] = (int16_t)w; wp.w[l][i][pl][1] = (int16_t)o;
-          }
-      }
-    if (!r.ok()) return PARSE_TRUNCATED;
-    if (st->profile == 66) return PARSE_INVALID;
-  }
-  const bool is_ref = nal.ref_idc != 0;                       // a non-reference picture is output but never predicted from
-  bool adaptive = false, idr_lt = false;
-  std::vector<ParsedPicture::Mmco> mmco;
-  if (nal.ref_idc) {                                          // dec_ref_pic_marking (7.3.3.3)
-    if (idr) { r.bit(); idr_lt = r.bit() != 0; }              // no_output_of_prior_pics_flag, long_term_reference_flag
-    else if (r.bit()) {
-      adaptive = true;
-      for (;;) {
-        ParsedPicture::Mmco m;
-        m.op = (int)r.ue(); m.a = m.b = 0;
-        if (m.op == 0) break;
-        if (m.op > 6 || !r.ok()) return PARSE_INVALID;
-        if (m.op == 1 || m.op == 3) m.a = (int)r.ue();        // difference_of_pic_nums_minus1
-        if (m.op == 2) m.a = (int)r.ue();                     // long_term_pic_num
-        if (m.op == 3 || m.op == 6) m.b = (int)r.ue();        // long_term_frame_idx
-        if (m.op == 4) m.a = (int)r.ue();                     // max_long_term_frame_idx_plus1
-        mmco.push_back(m);
-        if (mmco.size() > 64) return PARSE_INVALID;
-      }
-    }
-  }
-  int cabac_init_idc = 0;
-  if (st->entropy_cabac && inter_slice) {
+  // explicit weights of a P slice (weighted_pred_flag) or a B slice (weighted_bipred_idc 1)
+  if ((c.is_p && st->weighted_pred) || (c.is_b && st->weighted_bipred_idc == 1))
+    if ((rc = read_pred_weight_table(r, st, c)) != PARSE_OK) return rc;
+  c.is_ref = nal.ref_idc != 0;                                // a non-reference picture is output but never predicted from
+  if (c.is_ref && (rc = read_dec_ref_pic_marking(r, c)) != PARSE_OK) return rc;
+  if (st->entropy_cabac && c.inter) {
     const uint32_t v = r.ue();
     if (v > 2) return PARSE_INVALID;
-    cabac_init_idc = (int)v;
+    c.cabac_init_idc = (int)v;
   }
-  ss.qp = st->pic_init_qp + r.se();
-  int dbk_idc = 0, alpha_off = 0, beta_off = 0;
+  c.ss.qp = st->pic_init_qp + r.se();
   if (st->deblocking_control) {
-    dbk_idc = (int)r.ue();
-    if (dbk_idc > 2) return PARSE_INVALID;
-    if (dbk_idc != 1) {
-      alpha_off = 2 * r.se(); beta_off = 2 * r.se();
-      if (alpha_off < -12 || alpha_off > 12 || beta_off < -12 || beta_off > 12) return PARSE_INVALID;
+    c.dbk_idc = (int)r.ue();
+    if (c.dbk_idc > 2) return PARSE_INVALID;
+    if (c.dbk_idc != 1) {
+      c.alpha_off = 2 * r.se(); c.beta_off = 2 * r.se();
+      if (c.alpha_off < -12 || c.alpha_off > 12 || c.beta_off < -12 || c.beta_off > 12) return PARSE_INVALID;
     }
   }
   if (!r.ok()) return PARSE_TRUNCATED;
-  if (ss.qp < 0 || ss.qp > 51) return PARSE_INVALID;
-  if (idr) { if (ss.frame_num != 0) return PARSE_INVALID; }
-  else if (ss.frame_num != ((st->last_frame_num + 1) & ((1 << st->log2_max_frame_num) - 1))) return PARSE_UNSUPPORTED;   // a gap (7.4.3: frame_num
-                                                            // follows the last REFERENCE picture): needs error concealment
-  if (first_slice) {
-    pic->ss = ss;
-    pic->is_ref = is_ref;
-    pic->adaptive_marking = adaptive;
-    pic->mmco = mmco;
-    pic->idr_long_term = idr_lt;
-    pic->crop_left = 2 * st->crop_left; pic->crop_top = 2 * st->crop_top;
-    pic->n_slots = st->n_slots;
-    {                                                         // a slot no reference picture occupies
-      int slot = 0;
-      for (;; slot++) {
-        bool used = false;
-        if (!idr) for (const ParserState::RefPic& rp : st->refs) used = used || rp.slot == slot;
-        if (!used) break;
-      }
-      if (slot >= st->n_slots) return PARSE_INVALID;
-      pic->cur_slot = slot;
-    }
-    pic->disable_deblocking_idc = dbk_idc;
-    pic->poc = poc; pic->poc_msb = poc_msb; pic->poc_lsb = poc_lsb;
-    pic->pic_id = st->next_pic_id++;
-    pic->max_reorder = st->profile == 66 ? 0 : st->sp.num_ref_frames;
-    pic->has_b = false;
-    pic->has_t8 = st->transform_8x8; pic->chroma_qp_offset = st->chroma_qp_offset;
-    if (st->profile != 66) {                                  // the stream may hold B slices: keep the motion field of every picture
-      if ((int)st->motion.size() < st->n_slots) st->motion.resize(st->n_slots);
-      MotionStore& ms = st->motion[pic->cur_slot];
-      if ((int)ms.intra.size() != n) ms.size_for(n);
-      ms.poc = poc; ms.pic_id = pic->pic_id;
-    } else {
-      st->motion.clear();
-    }
-    // the records are initialised as the macroblocks are parsed (7.3 MB per 1080p picture are not filled up front: a skipped
-    // macroblock resets its 128 header bytes, a coded one its whole record); a picture is only handed out complete (next_mb == n)
-    if ((int)pic->mbs.size() != n) pic->mbs.assign(n, MbOut());
-    DecMbAux za;
-    memset(&za, 0, sizeof(za));
-    pic->aux.assign(n, za);
-  } else if (ss.idr != pic->ss.idr || ss.frame_num != pic->ss.frame_num || is_ref != pic->is_ref || poc != pic->poc) {
-    return PARSE_INVALID;                                     // slices of one access unit must agree
-  }
-  if ((is_b || wp.on) && !pic->has_b) {                       // B macroblocks, and P macroblocks with explicit weights, travel resolved
-    pic->has_b = true;
-    DecMbAuxB zb;
-    memset(&zb, 0, sizeof(zb));
-    pic->aux_b.assign(n, zb);
-  }
-  // host-side motion derivation (h264_motion.h): the field of every picture where B slices may occur, B macroblocks resolved here
-  MotionCtx M;
-  const bool track = !st->motion.empty();
-  if (track) { M.cur = &st->motion[pic->cur_slot]; M.mbw = mbw; }
-  BSliceCtx bsl;
-  if (is_b) {
-    bsl.direct_spatial = direct_spatial; bsl.cur_poc = poc; bsl.n_ref[0] = n_ref; bsl.n_ref[1] = n_ref1;
-    for (int l = 0; l < 2; l++) for (int i = 0; i < 33; i++) bsl.list[l][i] = lists[l][i];
-    bsl.implicit = st->weighted_bipred_idc == 2;
-    bsl.wp = wp.on ? &wp : nullptr;
-    bsl.cabac = st->entropy_cabac;
-    const int cslot = lists[1][0].slot;
-    bsl.col = (cslot >= 0 && cslot < (int)st->motion.size()) ? &st->motion[cslot] : nullptr;
-    bsl.col_long_term = lists[1][0].lt;
-  }
-  bool track_fail = false;
-  auto track_mb = [&](int i, const int* ri) {                 // a macroblock of an I / P slice is complete: its cells of the field
-    if (!track) return;
-    MbOut& mm = pic->mbs[i];
-    if (MBT_IS_INTRA(mm.mb_type)) M.store_intra(i);
-    else if (!MBT_IS_B(mm.mb_type)) {
-      derive_p(M, i, pic->aux[i].avail, mm, pic->aux[i], ri, lists[0]);
-      if (wp.on) {                                            // explicit weights: the macroblock travels resolved, like a B macroblock
-        if (!emit_resolved_p(M, lists[0], n_ref, wp, &pic->aux[i], &pic->aux_b[i])) track_fail = true;
-        mm.mb_type = mm.mb_type == MBT_PSKIP ? MBT_BSKIP : MBT_B;
-      }
-    }
-  };
-  static const int kRiZero[4] = {0, 0, 0, 0};
-  if (pic->n_slices >= 65535) return PARSE_UNSUPPORTED;
-  const int slice_no = pic->n_slices++;
-  if (dbk_idc != 1) pic->any_deblock = true;
+  if (c.ss.qp < 0 || c.ss.qp > 51) return PARSE_INVALID;
+  if (c.idr) { if (c.ss.frame_num != 0) return PARSE_INVALID; }
+  else if (c.ss.frame_num != ((st->last_frame_num + 1) & ((1 << st->log2_max_frame_num) - 1))) return PARSE_UNSUPPORTED;   // a gap (7.4.3:
+                                                            // frame_num follows the last REFERENCE picture): needs error concealment
+  return PARSE_OK;
+}
 
-  auto same_slice = [&](int other) { return other >= first_mb; };          // raster-ordered slices: a neighbour is in this slice iff it is not before its start
+// the first slice of a picture sets the picture up
+int start_picture(ParserState* st, ParsedPicture* pic, SliceCtx& c) {
+  pic->ss = c.ss;
+  pic->is_ref = c.is_ref;
+  pic->adaptive_marking = c.adaptive_marking;
+  pic->mmco = std::move(c.mmco);
+  pic->idr_long_term = c.idr_long_term;
+  pic->crop_left = 2 * st->crop_left; pic->crop_top = 2 * st->crop_top;
+  pic->n_slots = st->n_slots;
+  {                                                           // a slot no reference picture occupies
+    int slot = 0;
+    while (!c.idr && std::any_of(st->refs.begin(), st->refs.end(), [slot](const ParserState::RefPic& rp) { return rp.slot == slot; })) slot++;
+    if (slot >= st->n_slots) return PARSE_INVALID;
+    pic->cur_slot = slot;
+  }
+  pic->poc = c.poc; pic->poc_msb = c.poc_msb; pic->poc_lsb = c.poc_lsb;
+  pic->pic_id = st->next_pic_id++;
+  pic->max_reorder = st->profile == 66 ? 0 : st->sp.num_ref_frames;
+  pic->has_b = false;
+  pic->has_t8 = st->transform_8x8; pic->chroma_qp_offset = st->chroma_qp_offset;
+  const int n = st->sp.mb_w * st->sp.mb_h;
+  if (st->profile != 66) {                                    // the stream may hold B slices: keep the motion field of every picture
+    if ((int)st->motion.size() < st->n_slots) st->motion.resize(st->n_slots);
+    MotionStore& ms = st->motion[pic->cur_slot];
+    if ((int)ms.intra.size() != n) ms.size_for(n);
+    ms.poc = c.poc; ms.pic_id = pic->pic_id;
+  } else {
+    st->motion.clear();
+  }
+  // the records are initialised as the macroblocks are parsed (7.3 MB per 1080p picture are not filled up front: a skipped
+  // macroblock resets its 128 header bytes, a coded one its whole record); a picture is only handed out complete (next_mb == n)
+  if ((int)pic->mbs.size() != n) pic->mbs.assign(n, MbOut());
+  DecMbAux za;
+  memset(&za, 0, sizeof(za));
+  pic->aux.assign(n, za);
+  return PARSE_OK;
+}
 
-  // ---- slice data, CABAC (7.3.4 with entropy_coding_mode_flag = 1; macroblock layer 7.3.5, context selection 9.3.3.1.1) ----
-  if (st->entropy_cabac) {
-    while (r.pos() & 7) if (!r.bit()) return PARSE_INVALID;   // cabac_alignment_one_bit
-    if (!r.ok()) return PARSE_TRUNCATED;
-    CabacDecoder d(nal.rbsp.data(), nal.rbsp.size());
-    d.init_contexts(ss.qp, inter_slice ? 1 + cabac_init_idc : 0);
-    d.init_engine(r.pos());
-    if ((int)pic->cabac_info.size() != n) pic->cabac_info.resize(n);
-    CabacMbInfo* info = pic->cabac_info.data();
-    static const int kCbfOff[5] = {0, 4, 8, 12, 16};
-    int qp = ss.qp, idx = first_mb;
-    bool prev_dqp_nonzero = false;
-    for (;;) {
-      if (idx >= n) return PARSE_INVALID;                     // the slice goes on beyond the picture
-      const int mbx = idx % mbw, mby = idx / mbw;
-      const bool avL = mbx > 0 && same_slice(idx - 1), avT = mby > 0 && same_slice(idx - mbw);
-      const CabacMbInfo* L = avL ? &info[idx - 1] : nullptr;
-      const CabacMbInfo* T = avT ? &info[idx - mbw] : nullptr;
-      CabacMbInfo& me = info[idx];
-      memset(&me, 0, sizeof(me));
-      MbOut& m = pic->mbs[idx];
-      DecMbAux& ax = pic->aux[idx];
-      ax.slice = (uint16_t)slice_no; ax.dbk_idc = (uint8_t)dbk_idc; ax.alpha_off = (int8_t)alpha_off; ax.beta_off = (int8_t)beta_off;
-      ax.flags = st->constrained_intra_pred ? DECAUX_CIP : 0;
-      ax.avail = (uint8_t)((avL ? 1 : 0) | (avT ? 2 : 0) | (mbx > 0 && mby > 0 && same_slice(idx - mbw - 1) ? 4 : 0) |
-                           (mby > 0 && mbx < mbw - 1 && same_slice(idx - mbw + 1) ? 8 : 0));
-      int cur_ri[4] = {0, 0, 0, 0};                           // ref_idx_l0 of the 8x8 blocks of a P macroblock (host-side motion field)
-      if (inter_slice && d.decision((is_b ? 24 : 11) + (L && !L->skip ? 1 : 0) + (T && !T->skip ? 1 : 0))) {       // mb_skip_flag
-        reset_skip_record(&m);
-        m.qp = (uint8_t)qp;
-        ax.flags = 0;
-        if (is_b) {                                           // B_Skip: direct prediction, no residual
-          m.mb_type = MBT_BSKIP;
-          BMbSyntax sx;
-          sx.skip = true;
-          if (!derive_b(M, idx, ax.avail, sx, bsl, &ax, &pic->aux_b[idx])) return PARSE_INVALID;
-          me.type = MBT_BSKIP; me.skip = 1; me.direct = 1;
-        } else {
-          for (int q = 0; q < 4; q++) ax.ref_idx[q] = (int8_t)list0[0];
-          me.type = MBT_PSKIP; me.skip = 1;
+// the DecMbAux fields every macroblock carries: slice, deblocking control and which neighbours are available (slices come in
+// raster order, so a neighbour is in this slice iff it is not before the slice's first macroblock)
+DecMbAux& start_aux(const SliceCtx& c, int idx) {
+  DecMbAux& ax = c.pic->aux[idx];
+  const int w = c.mbw, x = idx % w, y = idx / w;
+  auto in_slice = [&](int other) { return other >= c.first_mb; };
+  ax.slice = (uint16_t)c.slice_no; ax.dbk_idc = (uint8_t)c.dbk_idc; ax.alpha_off = (int8_t)c.alpha_off; ax.beta_off = (int8_t)c.beta_off;
+  ax.avail = (uint8_t)((x > 0 && in_slice(idx - 1) ? 1 : 0) | (y > 0 && in_slice(idx - w) ? 2 : 0) |
+                       (x > 0 && y > 0 && in_slice(idx - w - 1) ? 4 : 0) | (y > 0 && x < w - 1 && in_slice(idx - w + 1) ? 8 : 0));
+  return ax;
+}
+
+// P_Skip (ref_idx 0, vector predicted later) or B_Skip (direct prediction): no residual, QP_Y carried over
+int skip_mb(SliceCtx& c, int idx, DecMbAux& ax, int qp) {
+  MbOut& m = c.pic->mbs[idx];
+  reset_skip_record(&m);
+  m.qp = (uint8_t)qp;
+  if (!c.is_b) {
+    for (int q = 0; q < 4; q++) ax.ref_idx[q] = (int8_t)c.lists[0][0].slot;
+    return PARSE_OK;
+  }
+  m.mb_type = MBT_BSKIP;
+  BMbSyntax sx;
+  sx.skip = true;
+  return derive_b(c.M, idx, ax.avail, sx, c.b, &ax, &c.pic->aux_b[idx]) ? PARSE_OK : PARSE_INVALID;
+}
+
+// mb_type of a P or B slice past its inter types is an intra type (Tables 7-13, 7-14): true, t becomes its I-slice number
+bool intra_mb_type(const SliceCtx& c, int* t) {
+  if (!c.inter) return true;
+  const int n_inter = c.is_p ? 5 : 23;
+  if (*t < n_inter) return false;
+  *t -= n_inter;
+  return true;
+}
+
+// I_16x16 mb_type t (Table 7-11): the prediction mode into the record; returns the coded_block_pattern it names
+int i16x16_record(MbOut& m, int t) {
+  m.mb_type = MBT_I16x16;
+  const int v = t - 1;
+  m.i16_mode = (uint8_t)(v & 3);
+  return (((v >> 2) % 3) << 4) | (v >= 12 ? 15 : 0);
+}
+
+// the intra prediction modes must have their neighbours (8.3.3, 8.3.4); with constrained intra prediction the construct stage
+// knows which count
+bool intra_modes_ok(const SliceCtx& c, const MbOut& m, int avail) {
+  if (m.chroma_mode > 3) return false;
+  if (c.st->constrained_intra_pred) return true;
+  const bool L = avail & 1, T = avail & 2;
+  if ((m.chroma_mode == 1 && !L) || (m.chroma_mode == 2 && !T) || (m.chroma_mode == 3 && !(L && T))) return false;
+  return !(m.mb_type == MBT_I16x16 && ((m.i16_mode == 0 && !T) || (m.i16_mode == 1 && !L) || (m.i16_mode == 3 && !(L && T))));
+}
+
+// I_PCM after its samples: every block counts as 16 coefficients for the neighbours' contexts (9.2.1), QP'Y is 0 for the deblocking
+// filter; like the reference decoder (decode_slice.cpp:1870: iLastMbQp untouched) the QP predictor of the next macroblock stays
+void pcm_record(MbOut& m) {
+  m.mb_type = MBT_IPCM;
+  for (int i = 0; i < 24; i++) m.nnz[i] = 16;
+  m.cbp = 0x2f;
+  m.qp = 0;
+}
+
+// P macroblock (7.3.5.1 / 7.3.5.2 of P slices): the partitions of mb_type t, their ref_idx_l0 (ri, and as picture slots in ax) and
+// their vectors, as the slice's entropy coder reads them.  read_sub() returns -1 for a value out of range; read_ref(q0, qmask) reads
+// the ref_idx of the 8x8 blocks in qmask (q0 the first); read_mvd(blk, w4, h4, int16_t v[2]) the vector of the partition whose
+// first 4x4 block is blk.
+template <class ReadSub, class ReadRef, class ReadMvd>
+int read_p_mb(const SliceCtx& c, int t, MbOut& m, DecMbAux& ax, int ri[4], bool* no_sub8, ReadSub read_sub, ReadRef read_ref, ReadMvd read_mvd) {
+  static const uint8_t kMask[3][2] = {{15, 0}, {3, 12}, {5, 10}};     // 8x8 blocks of the partitions of P_L0_16x16, _16x8, _8x16
+  static const uint8_t kPart[3][2][3] = {{{0, 4, 4}}, {{0, 4, 2}, {8, 4, 2}}, {{0, 2, 4}, {2, 2, 4}}};   // first 4x4 block, w4, h4
+  static const uint8_t kN[4] = {1, 2, 2, 4}, kW[4] = {2, 2, 1, 1}, kH[4] = {2, 1, 2, 1};   // per sub_mb_type: partitions, w4, h4
+  static const uint8_t kOff[4][4] = {{0}, {0, 4}, {0, 1}, {0, 1, 4, 5}};                  // their first 4x4 blocks in the 8x8
+  if (t < 0 || t > 4) return PARSE_INVALID;
+  const bool p8x8 = t >= 3;                                   // P_8x8, or P_8x8ref0 (t 4, CAVLC only: every reference index is 0)
+  const int np = t == 0 ? 1 : 2;
+  m.mb_type = t == 0 ? MBT_P16x16 : t == 1 ? MBT_P16x8 : t == 2 ? MBT_P8x16 : MBT_P8x8;
+  bool sub = false;
+  for (int k = 0; p8x8 && k < 4; k++) {
+    const int v = read_sub();
+    if (v < 0) return PARSE_INVALID;
+    ax.sub_type[k] = (uint8_t)v;
+    sub = sub || v != 0;
+  }
+  if (!p8x8)
+    for (int p = 0; p < np; p++) {
+      const int mask = kMask[t][p], v = read_ref(__builtin_ctz(mask), mask);
+      for (int q = 0; q < 4; q++) if (mask & (1 << q)) ri[q] = v;
+    }
+  else if (t == 3) for (int k = 0; k < 4; k++) ri[k] = read_ref(k, 1 << k);
+  for (int k = 0; k < 4; k++) {
+    if (ri[k] < 0 || ri[k] >= c.n_ref[0]) return PARSE_INVALID;
+    ax.ref_idx[k] = (int8_t)c.lists[0][ri[k]].slot;
+  }
+  if (!p8x8) {
+    for (int p = 0; p < np; p++) read_mvd(kPart[t][p][0], kPart[t][p][1], kPart[t][p][2], m.mvd[p]);
+    return PARSE_OK;
+  }
+  for (int k = 0; k < 4; k++) {
+    const int st = ax.sub_type[k], b0 = (k & 1) * 2 + (k >> 1) * 8;
+    for (int j = 0; j < kN[st]; j++) read_mvd(b0 + kOff[st][j], kW[st], kH[st], ax.mvd[4 * k + j]);
+  }
+  // with sub-macroblock partitions the vectors stay in ax.mvd; without, the record carries the four 8x8 vectors as the encoder's does
+  if (sub) { ax.flags |= DECAUX_SUB; *no_sub8 = false; }
+  else for (int k = 0; k < 4; k++) { m.mvd[k][0] = ax.mvd[4 * k][0]; m.mvd[k][1] = ax.mvd[4 * k][1]; }
+  return PARSE_OK;
+}
+
+// B macroblock (7.3.5.1 / 7.3.5.2 of B slices): sub_mb_type, ref_idx and mvd as the slice's entropy coder reads them, collected for
+// derive_b().  read_sub() returns -1 for a value out of range; read_ref(l, unit) and read_mvd(l, unit, int16_t v[2]) read one
+// partition's syntax element of list l.
+template <class ReadSub, class ReadRef, class ReadMvd>
+int read_b_mb(const SliceCtx& c, int t, MbOut& m, BMbSyntax& sx, bool* no_sub8, ReadSub read_sub, ReadRef read_ref, ReadMvd read_mvd) {
+  m.mb_type = MBT_B;
+  memset(sx.ref, 0, sizeof(sx.ref)); memset(sx.mvd, 0, sizeof(sx.mvd));
+  sx.type = t;
+  if (t == 22)
+    for (int k = 0; k < 4; k++) {
+      const int v = read_sub();
+      if (v < 0) return PARSE_INVALID;
+      sx.sub[k] = v;
+      if (v != 0 && b_sub_shape(v) != 0) *no_sub8 = false;
+    }
+  BUnit ru[4], mu[16];
+  const int nru = b_ref_units(sx, ru), nmu = b_mvd_units(sx, mu);
+  for (int l = 0; l < 2; l++)
+    for (int i = 0; i < nru; i++) {
+      if (!(ru[i].lists & (1 << l))) continue;
+      const int v = read_ref(l, ru[i]);
+      if (v < 0 || v >= c.n_ref[l]) return PARSE_INVALID;
+      for (int q = 0; q < 4; q++) if (ru[i].qmask & (1 << q)) sx.ref[l][q] = v;
+    }
+  for (int l = 0; l < 2; l++)
+    for (int i = 0; i < nmu; i++)
+      if (mu[i].lists & (1 << l)) read_mvd(l, mu[i], sx.mvd[l][mu[i].slot]);
+  return PARSE_OK;
+}
+
+// an I or P macroblock is complete: its motion field cells; with explicit weights a P macroblock travels resolved, like a B one
+void track_mb(SliceCtx& c, int i, const int ri[4]) {
+  if (!c.track) return;
+  MbOut& m = c.pic->mbs[i];
+  DecMbAux& ax = c.pic->aux[i];
+  if (MBT_IS_INTRA(m.mb_type)) c.M.store_intra(i);
+  else if (!MBT_IS_B(m.mb_type)) {
+    derive_p(c.M, i, ax.avail, m, ax, ri, c.lists[0]);
+    if (c.wp.on) {
+      if (!emit_resolved_p(c.M, c.lists[0], c.n_ref[0], c.wp, &ax, &c.pic->aux_b[i])) c.track_fail = true;
+      m.mb_type = m.mb_type == MBT_PSKIP ? MBT_BSKIP : MBT_B;
+    }
+  }
+}
+
+// ---- slice data, CABAC (7.3.4 with entropy_coding_mode_flag = 1; macroblock layer 7.3.5, context selection 9.3.3.1.1) ----
+
+// transform_size_8x8_flag
+int cabac_t8(CabacDecoder& d, const CabacMbInfo* L, const CabacMbInfo* T) {
+  return d.decision(399 + (L && L->t8 ? 1 : 0) + (T && T->t8 ? 1 : 0));
+}
+
+// ref_idx_lX of the 8x8 blocks in qmask, q0 the first: the context counts the blocks left of and above q0 with ref_idx > 0
+int cabac_ref_idx(CabacDecoder& d, const SliceCtx& c, CabacMbInfo& me, const CabacMbInfo* L, const CabacMbInfo* T, int l, int q0, int qmask) {
+  if (c.n_ref[l] <= 1) return 0;
+  uint8_t& gt = l ? me.ref_gt0_l1 : me.ref_gt0;
+  auto bits_of = [l](const CabacMbInfo* nb) { return nb ? (l ? nb->ref_gt0_l1 : nb->ref_gt0) : 0; };
+  const int qx = q0 & 1, qy = q0 >> 1;
+  const int a = qx ? (gt >> (q0 - 1)) & 1 : (bits_of(L) >> (qy * 2 + 1)) & 1;
+  const int b = qy ? (gt >> (q0 - 2)) & 1 : (bits_of(T) >> (2 + qx)) & 1;
+  const int v = d.ref_idx(a + 2 * b);
+  if (v > 0) gt |= (uint8_t)qmask;
+  return v;
+}
+
+// mvd_lX of the partition at 4x4 block (bx, by), w4 x h4 blocks: the context sums the neighbours' |mvd|, which it updates
+void cabac_mvd(CabacDecoder& d, CabacMbInfo& me, const CabacMbInfo* L, const CabacMbInfo* T, int l, int bx, int by, int w4, int h4, int16_t v[2]) {
+  uint8_t (*mine)[2] = l ? me.mvd_l1 : me.mvd;
+  int mv[2];
+  for (int c = 0; c < 2; c++) {
+    const int a = bx > 0 ? mine[by * 4 + bx - 1][c] : (L ? (l ? L->mvd_l1 : L->mvd)[by * 4 + 3][c] : 0);
+    const int b = by > 0 ? mine[(by - 1) * 4 + bx][c] : (T ? (l ? T->mvd_l1 : T->mvd)[12 + bx][c] : 0);
+    mv[c] = d.mvd(c ? 47 : 40, a + b);
+    v[c] = (int16_t)mv[c];
+  }
+  const uint8_t a0 = (uint8_t)(abs(mv[0]) > 255 ? 255 : abs(mv[0])), a1 = (uint8_t)(abs(mv[1]) > 255 ? 255 : abs(mv[1]));
+  for (int y = 0; y < h4; y++)
+    for (int x = 0; x < w4; x++) { mine[(by + y) * 4 + bx + x][0] = a0; mine[(by + y) * 4 + bx + x][1] = a1; }
+}
+
+// coded_block_flag of a neighbour's block (un: the value for a neighbour that is not available)
+inline int cbf_of(const CabacMbInfo* nb, int bit, int un) { return nb ? (int)((nb->cbf >> bit) & 1) : un; }
+
+// the residual of a macroblock with coded_block_pattern cbp (7.3.5.3 with CABAC)
+int cabac_residual(CabacDecoder& d, MbOut& m, CabacMbInfo& me, const CabacMbInfo* L, const CabacMbInfo* T, int cbp, bool intra, bool t8) {
+  static const int kCbfOff[5] = {0, 4, 8, 12, 16};
+  const int cbp_l = cbp & 15, cbp_c = cbp >> 4;
+  const int un = intra ? 1 : 0;                               // coded_block_flag of a block in a macroblock that is not available
+  if (m.mb_type == MBT_I16x16 && d.decision(85 + kCbfOff[0] + cbf_of(L, 24, un) + 2 * cbf_of(T, 24, un))) {
+    if (d.residual_levels(0, m.luma_dc, 16) < 0) return PARSE_INVALID;
+    me.cbf |= 1u << 24;
+  }
+  const int lcat = m.mb_type == MBT_I16x16 ? 1 : 2;
+  if (t8) {                                                   // four 8x8 blocks (ctxBlockCat 5: no coded_block_flag, the pattern bit decides)
+    for (int q = 0; q < 4; q++) {
+      if (!(cbp_l & (1 << q))) continue;
+      const int cnt = d.residual_levels8x8(&m.luma[4 * q][0]);
+      if (cnt < 0) return PARSE_INVALID;
+      const int b0 = (q >> 1) * 8 + (q & 1) * 2;
+      m.nnz[b0] = m.nnz[b0 + 1] = m.nnz[b0 + 4] = m.nnz[b0 + 5] = (int8_t)(cnt > 16 ? 16 : cnt);
+      me.cbf |= (1u << b0) | (1u << (b0 + 1)) | (1u << (b0 + 4)) | (1u << (b0 + 5));
+    }
+  }
+  for (int k = 0; k < 16 && !t8; k++) {
+    if (!(cbp_l & (1 << (k >> 2)))) continue;
+    const int bx = (k & 1) | ((k >> 1) & 2), by = ((k >> 1) & 1) | ((k >> 2) & 2);
+    const int a = bx > 0 ? (int)((me.cbf >> (by * 4 + bx - 1)) & 1) : cbf_of(L, by * 4 + 3, un);
+    const int b = by > 0 ? (int)((me.cbf >> ((by - 1) * 4 + bx)) & 1) : cbf_of(T, 12 + bx, un);
+    if (!d.decision(85 + kCbfOff[lcat] + a + 2 * b)) continue;
+    const int cnt = d.residual_levels(lcat, m.luma[k], lcat == 1 ? 15 : 16);
+    if (cnt < 0) return PARSE_INVALID;
+    m.nnz[by * 4 + bx] = (int8_t)cnt;
+    me.cbf |= 1u << (by * 4 + bx);
+  }
+  if (cbp_c) {
+    for (int uv = 0; uv < 2; uv++)
+      if (d.decision(85 + kCbfOff[3] + cbf_of(L, 25 + uv, un) + 2 * cbf_of(T, 25 + uv, un))) {
+        if (d.residual_levels(3, m.chroma_dc[uv], 4) < 0) return PARSE_INVALID;
+        me.cbf |= 1u << (25 + uv);
+      }
+    if (cbp_c == 2)
+      for (int uv = 0; uv < 2; uv++)
+        for (int j = 0; j < 4; j++) {
+          const int bx = j & 1, by = j >> 1, base = 16 + 4 * uv;
+          const int a = bx > 0 ? (int)((me.cbf >> (base + by * 2)) & 1) : cbf_of(L, base + by * 2 + 1, un);
+          const int b = by > 0 ? (int)((me.cbf >> (base + bx)) & 1) : cbf_of(T, base + 2 + bx, un);
+          if (!d.decision(85 + kCbfOff[4] + a + 2 * b)) continue;
+          const int cnt = d.residual_levels(4, m.chroma_ac[4 * uv + j], 15);
+          if (cnt < 0) return PARSE_INVALID;
+          m.nnz[base + j] = (int8_t)cnt;
+          me.cbf |= 1u << (base + j);
         }
+  }
+  return PARSE_OK;
+}
+
+int parse_slice_data_cabac(BitReader& r, const Nal& nal, SliceCtx& c) {
+  while (r.pos() & 7) if (!r.bit()) return PARSE_INVALID;     // cabac_alignment_one_bit
+  if (!r.ok()) return PARSE_TRUNCATED;
+  CabacDecoder d(nal.rbsp.data(), nal.rbsp.size());
+  d.init_contexts(c.ss.qp, c.inter ? 1 + c.cabac_init_idc : 0);
+  d.init_engine(r.pos());
+  ParsedPicture* pic = c.pic;
+  const int n = c.n_mb, mbw = c.mbw;
+  if ((int)pic->cabac_info.size() != n) pic->cabac_info.resize(n);
+  CabacMbInfo* info = pic->cabac_info.data();
+  int qp = c.ss.qp, idx = c.first_mb, rc;
+  bool prev_dqp_nonzero = false;
+  for (;;) {
+    if (idx >= n) return PARSE_INVALID;                       // the slice goes on beyond the picture
+    DecMbAux& ax = start_aux(c, idx);
+    const CabacMbInfo* L = (ax.avail & 1) ? &info[idx - 1] : nullptr;
+    const CabacMbInfo* T = (ax.avail & 2) ? &info[idx - mbw] : nullptr;
+    CabacMbInfo& me = info[idx];
+    memset(&me, 0, sizeof(me));
+    MbOut& m = pic->mbs[idx];
+    int ri[4] = {0, 0, 0, 0};                                 // ref_idx_l0 of the 8x8 blocks of a P macroblock (host-side motion field)
+    if (c.inter && d.decision((c.is_b ? 24 : 11) + (L && !L->skip ? 1 : 0) + (T && !T->skip ? 1 : 0))) {      // mb_skip_flag
+      if ((rc = skip_mb(c, idx, ax, qp)) != PARSE_OK) return rc;
+      me.type = m.mb_type; me.skip = 1; me.direct = c.is_b ? 1 : 0;
+      prev_dqp_nonzero = false;
+    } else {
+      memset(&m, 0, sizeof(m));
+      ax.flags = c.st->constrained_intra_pred ? DECAUX_CIP : 0;
+      int t = c.is_p ? d.mb_type_p()
+            : c.is_b ? d.mb_type_b((L && !L->direct ? 1 : 0) + (T && !T->direct ? 1 : 0))
+            : d.mb_type_intra(3 + (L && L->type != MBT_I4x4 ? 1 : 0) + (T && T->type != MBT_I4x4 ? 1 : 0), false);
+      const bool intra = intra_mb_type(c, &t);
+      me.intra = intra ? 1 : 0;
+      int cbp = -1;
+      bool no_sub8 = true;                                    // no sub-macroblock partition smaller than 8x8 (7.3.5: gate of transform_size_8x8_flag)
+      if (intra && t == 25) {                                 // I_PCM: the arithmetic decoder stopped behind its flush; raw bytes follow
+        size_t bp = (d.pos() + 7) & ~(size_t)7;               // pcm_alignment_zero_bit
+        const size_t byte0 = bp >> 3;
+        if (byte0 + 384 > nal.rbsp.size()) return PARSE_TRUNCATED;
+        memcpy(reinterpret_cast<uint8_t*>(m.luma), nal.rbsp.data() + byte0, 256);
+        memcpy(reinterpret_cast<uint8_t*>(m.chroma_ac), nal.rbsp.data() + byte0 + 256, 128);
+        d.init_engine(bp + 384 * 8);                          // 9.3.1.2: the engine starts over after the samples
+        pcm_record(m);
+        me.type = MBT_IPCM; me.cbp = 0x2f; me.cbf = 0x7ffffff;
         prev_dqp_nonzero = false;
       } else {
-        memset(&m, 0, sizeof(m));
-        int t;
-        bool intra = !inter_slice;
-        if (is_p) {
-          t = d.mb_type_p();
-          if (t >= 5) { intra = true; t -= 5; }
-        } else if (is_b) {
-          t = d.mb_type_b((L && !L->direct ? 1 : 0) + (T && !T->direct ? 1 : 0));
-          if (t >= 23) { intra = true; t -= 23; }
+        if (!intra && c.is_b) {                               // the syntax is collected, then resolved on the host (h264_motion.h)
+          if (t == 0) me.direct = 1;
+          BMbSyntax sx;
+          rc = read_b_mb(c, t, m, sx, &no_sub8, [&] { return d.sub_mb_type_b(); },
+                         [&](int l, const BUnit& u) { return cabac_ref_idx(d, c, me, L, T, l, u.q0, u.qmask); },
+                         [&](int l, const BUnit& u, int16_t* v) { cabac_mvd(d, me, L, T, l, u.bx, u.by, u.w4, u.h4, v); });
+          if (rc != PARSE_OK) return rc;
+          if (!d.ok()) return PARSE_TRUNCATED;
+          if (!derive_b(c.M, idx, ax.avail, sx, c.b, &ax, &c.pic->aux_b[idx])) return PARSE_INVALID;
+        } else if (!intra) {
+          rc = read_p_mb(c, t, m, ax, ri, &no_sub8, [&] { return d.sub_mb_type_p(); },
+                         [&](int q0, int qmask) { return cabac_ref_idx(d, c, me, L, T, 0, q0, qmask); },
+                         [&](int blk, int w4, int h4, int16_t* v) { cabac_mvd(d, me, L, T, 0, blk & 3, blk >> 2, w4, h4, v); });
+          if (rc != PARSE_OK) return rc;
         } else {
-          t = d.mb_type_intra(3 + (L && L->type != MBT_I4x4 ? 1 : 0) + (T && T->type != MBT_I4x4 ? 1 : 0), false);
+          if (t == 0) {
+            m.mb_type = MBT_I4x4;
+            const bool t8i = c.st->transform_8x8 && cabac_t8(d, L, T);        // Intra_8x8: four prediction modes instead of sixteen
+            if (t8i) { ax.flags |= DECAUX_T8; me.t8 = 1; }
+            for (int k = 0; k < (t8i ? 4 : 16); k++) {
+              m.prev_i4_flag[k] = (int8_t)d.decision(68);
+              if (!m.prev_i4_flag[k]) { int v = d.decision(69); v |= d.decision(69) << 1; v |= d.decision(69) << 2; m.rem_i4_mode[k] = (int8_t)v; }
+            }
+          } else {
+            cbp = i16x16_record(m, t);
+          }
+          m.chroma_mode = (uint8_t)d.intra_chroma_pred_mode((L && L->chroma_mode != 0 ? 1 : 0) + (T && T->chroma_mode != 0 ? 1 : 0));
+          me.chroma_mode = m.chroma_mode;
+          if (!intra_modes_ok(c, m, ax.avail)) return PARSE_INVALID;
         }
-        me.intra = intra ? 1 : 0;
-        int cbp = -1;
-        bool no_sub8 = true;                                  // no sub-macroblock partition smaller than 8x8 (7.3.5: gate of transform_size_8x8_flag)
-        auto read_t8 = [&]() { return d.decision(399 + (L && L->t8 ? 1 : 0) + (T && T->t8 ? 1 : 0)) != 0; };
-        if (intra && t == 25) {                               // I_PCM: the arithmetic decoder stopped behind its flush; raw bytes follow
-          m.mb_type = MBT_IPCM;
-          size_t bp = (d.pos() + 7) & ~(size_t)7;             // pcm_alignment_zero_bit
-          const size_t byte0 = bp >> 3;
-          if (byte0 + 384 > nal.rbsp.size()) return PARSE_TRUNCATED;
-          memcpy(reinterpret_cast<uint8_t*>(m.luma), nal.rbsp.data() + byte0, 256);
-          memcpy(reinterpret_cast<uint8_t*>(m.chroma_ac), nal.rbsp.data() + byte0 + 256, 128);
-          d.init_engine(bp + 384 * 8);                        // 9.3.1.2: the engine starts over after the samples
-          for (int i = 0; i < 24; i++) m.nnz[i] = 16;
-          m.cbp = 0x2f;
-          m.qp = 0;                                           // as in the CAVLC path: QP'Y 0 for the filter, the QP predictor stays
-          me.type = MBT_IPCM; me.cbp = 0x2f; me.cbf = 0x7ffffff;
+        me.type = m.mb_type;
+        if (cbp < 0) {                                        // coded_block_pattern: prefix (luma, 4 bins) + suffix (chroma)
+          const int la[2] = {L ? !((L->cbp >> 1) & 1) : 0, L ? !((L->cbp >> 3) & 1) : 0};
+          const int ta[2] = {T ? !((T->cbp >> 2) & 1) : 0, T ? !((T->cbp >> 3) & 1) : 0};
+          const int b0 = d.decision(73 + la[0] + 2 * ta[0]);
+          const int b1 = d.decision(73 + !b0 + 2 * ta[1]);
+          const int b2 = d.decision(73 + la[1] + 2 * !b0);
+          const int b3 = d.decision(73 + !b2 + 2 * !b1);
+          const int lc = L ? L->cbp >> 4 : 0, tc = T ? T->cbp >> 4 : 0;
+          int cc = d.decision(77 + (lc ? 1 : 0) + (tc ? 2 : 0));
+          if (cc) cc += d.decision(81 + (lc >> 1) + 2 * (tc >> 1));
+          cbp = b0 | (b1 << 1) | (b2 << 2) | (b3 << 3) | (cc << 4);
+        }
+        m.cbp = (uint8_t)cbp; me.cbp = (uint8_t)cbp;
+        if (!intra && (cbp & 15) && c.st->transform_8x8 && no_sub8 && cabac_t8(d, L, T)) { ax.flags |= DECAUX_T8; me.t8 = 1; }
+        if (cbp > 0 || m.mb_type == MBT_I16x16) {
+          const int dqp = d.mb_qp_delta(prev_dqp_nonzero ? 1 : 0);
+          if (dqp < -26 || dqp > 25) return PARSE_INVALID;
+          qp = (qp + dqp + 52) % 52;
+          prev_dqp_nonzero = dqp != 0;
+          if ((rc = cabac_residual(d, m, me, L, T, cbp, intra, (ax.flags & DECAUX_T8) != 0)) != PARSE_OK) return rc;
+        } else {
           prev_dqp_nonzero = false;
-        } else {
-          if (!intra && is_b) {
-            // B macroblock (7.3.5.1 / 7.3.5.2 for B slices): the syntax is collected, then resolved on the host (h264_motion.h)
-            m.mb_type = MBT_B;
-            BMbSyntax sx;
-            memset(sx.ref, 0, sizeof(sx.ref)); memset(sx.mvd, 0, sizeof(sx.mvd));
-            sx.type = t;
-            if (t == 0) me.direct = 1;
-            if (t == 22) for (int k = 0; k < 4; k++) { sx.sub[k] = d.sub_mb_type_b(); if (sx.sub[k] != 0 && b_sub_shape(sx.sub[k]) != 0) no_sub8 = false; }
-            BUnit ru[4], mu[16];
-            const int nru = b_ref_units(sx, ru), nmu = b_mvd_units(sx, mu);
-            for (int l = 0; l < 2; l++) {
-              const int nref_l = l ? n_ref1 : n_ref;
-              uint8_t& gt = l ? me.ref_gt0_l1 : me.ref_gt0;
-              for (int i = 0; i < nru; i++) {
-                if (!(ru[i].lists & (1 << l))) continue;
-                int v = 0;
-                if (nref_l > 1) {
-                  const int q = ru[i].q0, qx = q & 1, qy = q >> 1;
-                  auto bits_of = [&](const CabacMbInfo* nb) { return nb ? (l ? nb->ref_gt0_l1 : nb->ref_gt0) : 0; };
-                  const int a = qx ? (gt >> (q - 1)) & 1 : (bits_of(L) >> (qy * 2 + 1)) & 1;
-                  const int b = qy ? (gt >> (q - 2)) & 1 : (bits_of(T) >> (2 + qx)) & 1;
-                  v = d.ref_idx(a + 2 * b);
-                }
-                if (v >= nref_l) return PARSE_INVALID;
-                for (int q = 0; q < 4; q++) if (ru[i].qmask & (1 << q)) sx.ref[l][q] = v;
-                if (v > 0) gt |= (uint8_t)ru[i].qmask;
-              }
-            }
-            for (int l = 0; l < 2; l++) {
-              uint8_t (*mine)[2] = l ? me.mvd_l1 : me.mvd;
-              for (int i = 0; i < nmu; i++) {
-                if (!(mu[i].lists & (1 << l))) continue;
-                const int bx = mu[i].bx, by = mu[i].by;
-                int v[2];
-                for (int c = 0; c < 2; c++) {
-                  const int a = bx > 0 ? mine[by * 4 + bx - 1][c] : (L ? (l ? L->mvd_l1 : L->mvd)[by * 4 + 3][c] : 0);
-                  const int b = by > 0 ? mine[(by - 1) * 4 + bx][c] : (T ? (l ? T->mvd_l1 : T->mvd)[12 + bx][c] : 0);
-                  v[c] = d.mvd(c ? 47 : 40, a + b);
-                }
-                sx.mvd[l][mu[i].slot][0] = (int16_t)v[0]; sx.mvd[l][mu[i].slot][1] = (int16_t)v[1];
-                const uint8_t a0 = (uint8_t)(abs(v[0]) > 255 ? 255 : abs(v[0])), a1 = (uint8_t)(abs(v[1]) > 255 ? 255 : abs(v[1]));
-                for (int y = 0; y < mu[i].h4; y++)
-                  for (int x = 0; x < mu[i].w4; x++) { mine[(by + y) * 4 + bx + x][0] = a0; mine[(by + y) * 4 + bx + x][1] = a1; }
-              }
-            }
-            if (!d.ok()) return PARSE_TRUNCATED;
-            if (!derive_b(M, idx, ax.avail, sx, bsl, &ax, &pic->aux_b[idx])) return PARSE_INVALID;
-          } else if (!intra) {
-            int ri[4] = {0, 0, 0, 0};
-            // partitions as (first 4x4 block, width, height in 4x4 blocks); a P_8x8 macroblock lists its sub-macroblock partitions
-            struct Part { int b, w, h, q, slot; };             // q: 8x8 quadrant; slot: where the vector goes (m.mvd / ax.mvd index)
-            Part parts[16];
-            int np = 0;
-            if (t == 0) { m.mb_type = MBT_P16x16; parts[np++] = {0, 4, 4, 0, 0}; }
-            else if (t == 1) { m.mb_type = MBT_P16x8; parts[np++] = {0, 4, 2, 0, 0}; parts[np++] = {8, 4, 2, 2, 1}; }
-            else if (t == 2) { m.mb_type = MBT_P8x16; parts[np++] = {0, 2, 4, 0, 0}; parts[np++] = {2, 2, 4, 1, 1}; }
-            else {
-              m.mb_type = MBT_P8x8;
-              bool sub = false;
-              for (int k = 0; k < 4; k++) { ax.sub_type[k] = (uint8_t)d.sub_mb_type_p(); sub = sub || ax.sub_type[k] != 0; }
-              if (sub) { ax.flags |= DECAUX_SUB; no_sub8 = false; }
-              for (int k = 0; k < 4; k++) {
-                const int b0 = (k & 1) * 2 + (k >> 1) * 8;
-                switch (ax.sub_type[k]) {
-                  case 0: parts[np++] = {b0, 2, 2, k, 4 * k}; break;
-                  case 1: parts[np++] = {b0, 2, 1, k, 4 * k}; parts[np++] = {b0 + 4, 2, 1, k, 4 * k + 1}; break;
-                  case 2: parts[np++] = {b0, 1, 2, k, 4 * k}; parts[np++] = {b0 + 1, 1, 2, k, 4 * k + 1}; break;
-                  default:
-                    parts[np++] = {b0, 1, 1, k, 4 * k}; parts[np++] = {b0 + 1, 1, 1, k, 4 * k + 1};
-                    parts[np++] = {b0 + 4, 1, 1, k, 4 * k + 2}; parts[np++] = {b0 + 5, 1, 1, k, 4 * k + 3};
-                    break;
-                }
-              }
-            }
-            // ref_idx_l0 of every macroblock partition / sub-macroblock, then the vectors (7.3.5.1, 7.3.5.2)
-            if (n_ref > 1) {
-              auto gt0 = [&](int q) {                          // condTermFlag of the 8x8 blocks left of and above quadrant q
-                const int qx = q & 1, qy = q >> 1;
-                const int a = qx ? (me.ref_gt0 >> (q - 1)) & 1 : (L ? (L->ref_gt0 >> (qy * 2 + 1)) & 1 : 0);
-                const int b = qy ? (me.ref_gt0 >> (q - 2)) & 1 : (T ? (T->ref_gt0 >> (2 + qx)) & 1 : 0);
-                return a + 2 * b;
-              };
-              if (m.mb_type == MBT_P8x8) {
-                for (int k = 0; k < 4; k++) { ri[k] = d.ref_idx(gt0(k)); if (ri[k] > 0) me.ref_gt0 |= (uint8_t)(1 << k); }
-              } else {
-                const int nmp = m.mb_type == MBT_P16x16 ? 1 : 2;
-                for (int pi = 0; pi < nmp; pi++) {
-                  const int q0 = parts[pi].q;
-                  const int v = d.ref_idx(gt0(q0));
-                  const int mask = m.mb_type == MBT_P16x16 ? 15 : m.mb_type == MBT_P16x8 ? (3 << (2 * pi)) : (5 << pi);
-                  for (int q = 0; q < 4; q++) if (mask & (1 << q)) ri[q] = v;
-                  if (v > 0) me.ref_gt0 |= (uint8_t)mask;
-                }
-              }
-            }
-            for (int k = 0; k < 4; k++) {
-              if (ri[k] < 0 || ri[k] >= n_ref) return PARSE_INVALID;
-              ax.ref_idx[k] = (int8_t)list0[ri[k]];
-              cur_ri[k] = ri[k];
-            }
-            for (int pi = 0; pi < np; pi++) {
-              const Part& pt = parts[pi];
-              const int bx = pt.b & 3, by = pt.b >> 2;
-              int v[2];
-              for (int c = 0; c < 2; c++) {
-                const int a = bx > 0 ? me.mvd[pt.b - 1][c] : (L ? L->mvd[by * 4 + 3][c] : 0);
-                const int b = by > 0 ? me.mvd[pt.b - 4][c] : (T ? T->mvd[12 + bx][c] : 0);
-                v[c] = d.mvd(c ? 47 : 40, a + b);
-              }
-              if (m.mb_type == MBT_P8x8) { ax.mvd[pt.slot][0] = (int16_t)v[0]; ax.mvd[pt.slot][1] = (int16_t)v[1]; }
-              else { m.mvd[pt.slot][0] = (int16_t)v[0]; m.mvd[pt.slot][1] = (int16_t)v[1]; }
-              const uint8_t a0 = (uint8_t)(abs(v[0]) > 255 ? 255 : abs(v[0])), a1 = (uint8_t)(abs(v[1]) > 255 ? 255 : abs(v[1]));
-              for (int y = 0; y < pt.h; y++)
-                for (int x = 0; x < pt.w; x++) { me.mvd[(by + y) * 4 + bx + x][0] = a0; me.mvd[(by + y) * 4 + bx + x][1] = a1; }
-            }
-            if (m.mb_type == MBT_P8x8 && !(ax.flags & DECAUX_SUB))
-              for (int k = 0; k < 4; k++) { m.mvd[k][0] = ax.mvd[4 * k][0]; m.mvd[k][1] = ax.mvd[4 * k][1]; }
-          } else {
-            if (t == 0) {
-              m.mb_type = MBT_I4x4;
-              const bool t8i = st->transform_8x8 && read_t8();          // Intra_8x8: four prediction modes instead of sixteen
-              if (t8i) { ax.flags |= DECAUX_T8; me.t8 = 1; }
-              for (int k = 0; k < (t8i ? 4 : 16); k++) {
-                m.prev_i4_flag[k] = (int8_t)d.decision(68);
-                if (!m.prev_i4_flag[k]) { int v = d.decision(69); v |= d.decision(69) << 1; v |= d.decision(69) << 2; m.rem_i4_mode[k] = (int8_t)v; }
-              }
-            } else {
-              m.mb_type = MBT_I16x16;
-              const int v = t - 1;
-              m.i16_mode = (uint8_t)(v & 3);
-              cbp = (((v >> 2) % 3) << 4) | (v >= 12 ? 15 : 0);
-            }
-            m.chroma_mode = (uint8_t)d.intra_chroma_pred_mode((L && L->chroma_mode != 0 ? 1 : 0) + (T && T->chroma_mode != 0 ? 1 : 0));
-            me.chroma_mode = m.chroma_mode;
-            if (!st->constrained_intra_pred) {
-              if ((m.chroma_mode == 1 && !avL) || (m.chroma_mode == 2 && !avT) || (m.chroma_mode == 3 && !(avL && avT))) return PARSE_INVALID;
-              if (m.mb_type == MBT_I16x16 &&
-                  ((m.i16_mode == 0 && !avT) || (m.i16_mode == 1 && !avL) || (m.i16_mode == 3 && !(avL && avT)))) return PARSE_INVALID;
-            }
-          }
-          me.type = m.mb_type;
-          if (cbp < 0) {                                      // coded_block_pattern: prefix (luma, 4 bins) + suffix (chroma)
-            const int la[2] = {L ? !((L->cbp >> 1) & 1) : 0, L ? !((L->cbp >> 3) & 1) : 0};
-            const int ta[2] = {T ? !((T->cbp >> 2) & 1) : 0, T ? !((T->cbp >> 3) & 1) : 0};
-            const int b0 = d.decision(73 + la[0] + 2 * ta[0]);
-            const int b1 = d.decision(73 + !b0 + 2 * ta[1]);
-            const int b2 = d.decision(73 + la[1] + 2 * !b0);
-            const int b3 = d.decision(73 + !b2 + 2 * !b1);
-            const int lc = L ? L->cbp >> 4 : 0, tc = T ? T->cbp >> 4 : 0;
-            int cc = d.decision(77 + (lc ? 1 : 0) + (tc ? 2 : 0));
-            if (cc) cc += d.decision(81 + (lc >> 1) + 2 * (tc >> 1));
-            cbp = b0 | (b1 << 1) | (b2 << 2) | (b3 << 3) | (cc << 4);
-          }
-          m.cbp = (uint8_t)cbp; me.cbp = (uint8_t)cbp;
-          const int cbp_l = cbp & 15, cbp_c = cbp >> 4;
-          if (!intra && cbp_l > 0 && st->transform_8x8 && no_sub8 && read_t8()) { ax.flags |= DECAUX_T8; me.t8 = 1; }
-          const bool t8 = (ax.flags & DECAUX_T8) != 0;
-          if (cbp > 0 || m.mb_type == MBT_I16x16) {
-            const int dqp = d.mb_qp_delta(prev_dqp_nonzero ? 1 : 0);
-            if (dqp < -26 || dqp > 25) return PARSE_INVALID;
-            qp = (qp + dqp + 52) % 52;
-            prev_dqp_nonzero = dqp != 0;
-            const int un = intra ? 1 : 0;                     // coded_block_flag of a block in a macroblock that is not available
-            auto cbf_of = [&](const CabacMbInfo* nb, int bit) { return nb ? (int)((nb->cbf >> bit) & 1) : un; };
-            auto luma_inc = [&](int bx, int by) {
-              const int a = bx > 0 ? (int)((me.cbf >> (by * 4 + bx - 1)) & 1) : cbf_of(L, by * 4 + 3);
-              const int b = by > 0 ? (int)((me.cbf >> ((by - 1) * 4 + bx)) & 1) : cbf_of(T, 12 + bx);
-              return a + 2 * b;
-            };
-            if (m.mb_type == MBT_I16x16 && d.decision(85 + kCbfOff[0] + cbf_of(L, 24) + 2 * cbf_of(T, 24))) {
-              if (d.residual_levels(0, m.luma_dc, 16) < 0) return PARSE_INVALID;
-              me.cbf |= 1u << 24;
-            }
-            const int lcat = m.mb_type == MBT_I16x16 ? 1 : 2;
-            if (t8) {                                         // four 8x8 blocks (ctxBlockCat 5: no coded_block_flag, the pattern bit decides)
-              for (int q = 0; q < 4; q++) {
-                if (!(cbp_l & (1 << q))) continue;
-                const int cnt = d.residual_levels8x8(&m.luma[4 * q][0]);
-                if (cnt < 0) return PARSE_INVALID;
-                const int b0 = (q >> 1) * 8 + (q & 1) * 2;
-                m.nnz[b0] = m.nnz[b0 + 1] = m.nnz[b0 + 4] = m.nnz[b0 + 5] = (int8_t)(cnt > 16 ? 16 : cnt);
-                me.cbf |= (1u << b0) | (1u << (b0 + 1)) | (1u << (b0 + 4)) | (1u << (b0 + 5));
-              }
-            }
-            for (int k = 0; k < 16 && !t8; k++) {
-              if (!(cbp_l & (1 << (k >> 2)))) continue;
-              const int bx = (k & 1) | ((k >> 1) & 2), by = ((k >> 1) & 1) | ((k >> 2) & 2);
-              if (!d.decision(85 + kCbfOff[lcat] + luma_inc(bx, by))) continue;
-              const int cnt = d.residual_levels(lcat, m.luma[k], lcat == 1 ? 15 : 16);
-              if (cnt < 0) return PARSE_INVALID;
-              m.nnz[by * 4 + bx] = (int8_t)cnt;
-              me.cbf |= 1u << (by * 4 + bx);
-            }
-            if (cbp_c) {
-              for (int uv = 0; uv < 2; uv++)
-                if (d.decision(85 + kCbfOff[3] + cbf_of(L, 25 + uv) + 2 * cbf_of(T, 25 + uv))) {
-                  if (d.residual_levels(3, m.chroma_dc[uv], 4) < 0) return PARSE_INVALID;
-                  me.cbf |= 1u << (25 + uv);
-                }
-              if (cbp_c == 2)
-                for (int uv = 0; uv < 2; uv++)
-                  for (int j = 0; j < 4; j++) {
-                    const int bx = j & 1, by = j >> 1, base = 16 + 4 * uv;
-                    const int a = bx > 0 ? (int)((me.cbf >> (base + by * 2)) & 1) : cbf_of(L, base + by * 2 + 1);
-                    const int b = by > 0 ? (int)((me.cbf >> (base + bx)) & 1) : cbf_of(T, base + 2 + bx);
-                    if (!d.decision(85 + kCbfOff[4] + a + 2 * b)) continue;
-                    const int cnt = d.residual_levels(4, m.chroma_ac[4 * uv + j], 15);
-                    if (cnt < 0) return PARSE_INVALID;
-                    m.nnz[base + j] = (int8_t)cnt;
-                    me.cbf |= 1u << (base + j);
-                  }
-            }
-          } else {
-            prev_dqp_nonzero = false;
-          }
-          m.qp = (uint8_t)qp;
         }
+        m.qp = (uint8_t)qp;
       }
-      if (!d.ok()) return PARSE_TRUNCATED;
-      track_mb(idx, cur_ri);
-      idx++;
-      if (d.terminate()) break;                               // end_of_slice_flag
     }
-    pic->next_mb = idx;
-    return track_fail ? PARSE_INVALID : PARSE_OK;
+    if (!d.ok()) return PARSE_TRUNCATED;
+    track_mb(c, idx, ri);
+    idx++;
+    if (d.terminate()) break;                                 // end_of_slice_flag
   }
+  pic->next_mb = idx;
+  return PARSE_OK;
+}
 
-  // ---- slice data, CAVLC ----
-  int qp = ss.qp;
-  int idx = first_mb;
+// ---- slice data, CAVLC ----
+
+// te(v) of a reference index with range num_ref_idx_active - 1 (9.1): absent for one picture, an inverted bit for two, else ue(v)
+inline int read_te(BitReader& r, int n_ref) { return n_ref == 1 ? 0 : n_ref == 2 ? !r.bit() : (int)r.ue(); }
+
+int parse_slice_data_cavlc(BitReader& r, SliceCtx& c) {
+  static const int kRiZero[4] = {0, 0, 0, 0};
+  ParsedPicture* pic = c.pic;
+  const int n = c.n_mb, mbw = c.mbw;
+  int qp = c.ss.qp, idx = c.first_mb, rc;
   while (idx < n) {
-    if (inter_slice) {
-      const int run = (int)r.ue();
+    if (c.inter) {
+      const int run = (int)r.ue();                            // mb_skip_run
       if (!r.ok() || idx + run > n) return PARSE_INVALID;
       for (int k = 0; k < run; k++, idx++) {
-        reset_skip_record(&pic->mbs[idx]);
-        pic->mbs[idx].qp = (uint8_t)qp;
-        DecMbAux& a = pic->aux[idx];
-        a.slice = (uint16_t)slice_no; a.dbk_idc = (uint8_t)dbk_idc; a.alpha_off = (int8_t)alpha_off; a.beta_off = (int8_t)beta_off;
-        const int x = idx % mbw, y = idx / mbw;
-        a.avail = (uint8_t)((x > 0 && same_slice(idx - 1) ? 1 : 0) | (y > 0 && same_slice(idx - mbw) ? 2 : 0) |
-                            (x > 0 && y > 0 && same_slice(idx - mbw - 1) ? 4 : 0) | (y > 0 && x < mbw - 1 && same_slice(idx - mbw + 1) ? 8 : 0));
-        if (is_b) {                                           // B_Skip
-          pic->mbs[idx].mb_type = MBT_BSKIP;
-          BMbSyntax sx;
-          sx.skip = true;
-          if (!derive_b(M, idx, a.avail, sx, bsl, &a, &pic->aux_b[idx])) return PARSE_INVALID;
-        } else {
-          for (int q = 0; q < 4; q++) a.ref_idx[q] = (int8_t)list0[0];
-          track_mb(idx, kRiZero);
-        }
+        if ((rc = skip_mb(c, idx, start_aux(c, idx), qp)) != PARSE_OK) return rc;
+        track_mb(c, idx, kRiZero);
       }
       if (idx == n || !r.more_data()) break;                  // the slice may end with a skip run
     }
     MbOut& m = pic->mbs[idx];
     memset(&m, 0, sizeof(m));
-    m.mb_type = MBT_PSKIP;
-    DecMbAux& ax = pic->aux[idx];
-    const int mbx = idx % mbw, mby = idx / mbw;
-    ax.slice = (uint16_t)slice_no; ax.dbk_idc = (uint8_t)dbk_idc; ax.alpha_off = (int8_t)alpha_off; ax.beta_off = (int8_t)beta_off;
-    ax.flags = st->constrained_intra_pred ? DECAUX_CIP : 0;
-    const bool avL = mbx > 0 && same_slice(idx - 1), avT = mby > 0 && same_slice(idx - mbw);
-    ax.avail = (uint8_t)((avL ? 1 : 0) | (avT ? 2 : 0) | (mbx > 0 && mby > 0 && same_slice(idx - mbw - 1) ? 4 : 0) |
-                         (mby > 0 && mbx < mbw - 1 && same_slice(idx - mbw + 1) ? 8 : 0));
+    DecMbAux& ax = start_aux(c, idx);
+    ax.flags = c.st->constrained_intra_pred ? DECAUX_CIP : 0;
     int t = (int)r.ue();
-    bool intra = !inter_slice;
-    if (is_p) {
-      if (t >= 5) { intra = true; t -= 5; }
-    } else if (is_b) {
-      if (t >= 23) { intra = true; t -= 23; }
-    }
-    int cbp = -1;
-    int cur_ri[4] = {0, 0, 0, 0};
+    const bool intra = intra_mb_type(c, &t);
+    int cbp = -1, ri[4] = {0, 0, 0, 0};
     bool no_sub8 = true;
-    if (!intra && is_b) {
-      // B macroblock: the syntax is collected (mb_pred / sub_mb_pred of B slices), then resolved on the host (h264_motion.h)
-      m.mb_type = MBT_B;
+    if (!intra && c.is_b) {                                   // the syntax is collected, then resolved on the host (h264_motion.h)
       BMbSyntax sx;
-      memset(sx.ref, 0, sizeof(sx.ref)); memset(sx.mvd, 0, sizeof(sx.mvd));
-      sx.type = t;
-      if (t == 22)
-        for (int k = 0; k < 4; k++) {
-          const uint32_t v = r.ue();
-          if (v > 12) return PARSE_INVALID;
-          sx.sub[k] = (int)v;
-          if (v != 0 && b_sub_shape((int)v) != 0) no_sub8 = false;
-        }
-      BUnit ru[4], mu[16];
-      const int nru = b_ref_units(sx, ru), nmu = b_mvd_units(sx, mu);
-      for (int l = 0; l < 2; l++) {
-        const int nref_l = l ? n_ref1 : n_ref;
-        for (int i = 0; i < nru; i++) {
-          if (!(ru[i].lists & (1 << l))) continue;
-          const int v = nref_l == 1 ? 0 : nref_l == 2 ? !r.bit() : (int)r.ue();       // te(v)
-          if (v < 0 || v >= nref_l) return PARSE_INVALID;
-          for (int q = 0; q < 4; q++) if (ru[i].qmask & (1 << q)) sx.ref[l][q] = v;
-        }
-      }
-      for (int l = 0; l < 2; l++)
-        for (int i = 0; i < nmu; i++) {
-          if (!(mu[i].lists & (1 << l))) continue;
-          sx.mvd[l][mu[i].slot][0] = (int16_t)r.se(); sx.mvd[l][mu[i].slot][1] = (int16_t)r.se();
-        }
+      rc = read_b_mb(c, t, m, sx, &no_sub8, [&] { const uint32_t v = r.ue(); return v > 12 ? -1 : (int)v; },
+                     [&](int l, const BUnit&) { return read_te(r, c.n_ref[l]); },
+                     [&](int, const BUnit&, int16_t* v) { v[0] = (int16_t)r.se(); v[1] = (int16_t)r.se(); });
+      if (rc != PARSE_OK) return rc;
       if (!r.ok()) return PARSE_TRUNCATED;
-      if (!derive_b(M, idx, ax.avail, sx, bsl, &ax, &pic->aux_b[idx])) return PARSE_INVALID;
+      if (!derive_b(c.M, idx, ax.avail, sx, c.b, &ax, &c.pic->aux_b[idx])) return PARSE_INVALID;
     } else if (!intra) {
-      // ref_idx_l0: te(v) with range num_ref_idx_active - 1 (9.1): absent for one picture, an inverted bit for two, else ue(v)
-      auto read_ref = [&]() -> int {
-        if (n_ref == 1) return 0;
-        const int v = n_ref == 2 ? !r.bit() : (int)r.ue();
-        return v;
-      };
-      int ri[4] = {0, 0, 0, 0};
-      if (t == 0) {
-        m.mb_type = MBT_P16x16;
-        ri[0] = ri[1] = ri[2] = ri[3] = read_ref();
-        m.mvd[0][0] = (int16_t)r.se(); m.mvd[0][1] = (int16_t)r.se();
-      } else if (t == 1 || t == 2) {
-        m.mb_type = t == 1 ? MBT_P16x8 : MBT_P8x16;
-        const int r0 = read_ref(), r1 = read_ref();
-        if (t == 1) { ri[0] = ri[1] = r0; ri[2] = ri[3] = r1; } else { ri[0] = ri[2] = r0; ri[1] = ri[3] = r1; }
-        for (int k = 0; k < 2; k++) { m.mvd[k][0] = (int16_t)r.se(); m.mvd[k][1] = (int16_t)r.se(); }
-      } else if (t == 3 || t == 4) {                          // P_8x8 / P_8x8ref0 (the latter: every reference index is 0)
-        m.mb_type = MBT_P8x8;
-        bool sub = false;
-        for (int k = 0; k < 4; k++) {
-          const uint32_t v = r.ue();
-          if (v > 3) return PARSE_INVALID;
-          ax.sub_type[k] = (uint8_t)v;
-          sub = sub || v != 0;
-        }
-        if (t == 3) for (int k = 0; k < 4; k++) ri[k] = read_ref();
-        static const int kParts[4] = {1, 2, 2, 4};
-        for (int k = 0; k < 4; k++)
-          for (int j = 0; j < kParts[ax.sub_type[k]]; j++) { ax.mvd[4 * k + j][0] = (int16_t)r.se(); ax.mvd[4 * k + j][1] = (int16_t)r.se(); }
-        if (sub) { ax.flags |= DECAUX_SUB; no_sub8 = false; }
-        else for (int k = 0; k < 4; k++) { m.mvd[k][0] = ax.mvd[4 * k][0]; m.mvd[k][1] = ax.mvd[4 * k][1]; }
-      } else return PARSE_INVALID;
-      for (int k = 0; k < 4; k++) {
-        if (ri[k] < 0 || ri[k] >= n_ref) return PARSE_INVALID;
-        ax.ref_idx[k] = (int8_t)list0[ri[k]];
-        cur_ri[k] = ri[k];
-      }
+      rc = read_p_mb(c, t, m, ax, ri, &no_sub8, [&] { const uint32_t v = r.ue(); return v > 3 ? -1 : (int)v; },
+                     [&](int, int) { return read_te(r, c.n_ref[0]); },
+                     [&](int, int, int, int16_t* v) { v[0] = (int16_t)r.se(); v[1] = (int16_t)r.se(); });
+      if (rc != PARSE_OK) return rc;
     } else {
       if (t == 0) {
         m.mb_type = MBT_I4x4;
-        const bool t8i = st->transform_8x8 && r.bit();        // transform_size_8x8_flag: Intra_8x8, four prediction modes
+        const bool t8i = c.st->transform_8x8 && r.bit();      // transform_size_8x8_flag: Intra_8x8, four prediction modes
         if (t8i) ax.flags |= DECAUX_T8;
         for (int k = 0; k < (t8i ? 4 : 16); k++) { m.prev_i4_flag[k] = (int8_t)r.bit(); m.rem_i4_mode[k] = m.prev_i4_flag[k] ? 0 : (int8_t)r.get(3); }
-        m.chroma_mode = (uint8_t)r.ue();
       } else if (t <= 24) {
-        m.mb_type = MBT_I16x16;
-        const int v = t - 1;
-        m.i16_mode = (uint8_t)(v & 3);
-        cbp = (((v >> 2) % 3) << 4) | (v >= 12 ? 15 : 0);
-        m.chroma_mode = (uint8_t)r.ue();
+        cbp = i16x16_record(m, t);
       } else if (t == 25) {                                   // I_PCM (7.3.5): byte-aligned raw samples
-        m.mb_type = MBT_IPCM;
         while (r.pos() & 7) r.skip(1);
         uint8_t* py = reinterpret_cast<uint8_t*>(m.luma);
         uint8_t* pc = reinterpret_cast<uint8_t*>(m.chroma_ac);
         for (int i = 0; i < 256; i++) py[i] = (uint8_t)r.get(8);
         for (int i = 0; i < 128; i++) pc[i] = (uint8_t)r.get(8);
         if (!r.ok()) return PARSE_TRUNCATED;
-        for (int i = 0; i < 24; i++) m.nnz[i] = 16;           // what the neighbours' coeff_token context sees (9.2.1)
-        m.cbp = 0x2f;
-        m.qp = 0;                                             // QP'Y of an I_PCM macroblock is 0 for the deblocking filter; like the reference
-                                                              // decoder (decode_slice.cpp:1870: iLastMbQp untouched) the QP predictor
-                                                              // of the next macroblock stays what it was
-        track_mb(idx, kRiZero);
+        pcm_record(m);
+        track_mb(c, idx, kRiZero);
         idx++;
         if (!r.more_data()) break;
         continue;
       } else return PARSE_INVALID;
-      if (m.chroma_mode > 3) return PARSE_INVALID;
-      if (!st->constrained_intra_pred) {                      // prediction modes must have their neighbours (8.3.3, 8.3.4); with
-        const bool L = avL, T = avT;                          // constrained intra prediction the construct stage knows which count
-        if ((m.chroma_mode == 1 && !L) || (m.chroma_mode == 2 && !T) || (m.chroma_mode == 3 && !(L && T))) return PARSE_INVALID;
-        if (m.mb_type == MBT_I16x16 &&
-            ((m.i16_mode == 0 && !T) || (m.i16_mode == 1 && !L) || (m.i16_mode == 3 && !(L && T)))) return PARSE_INVALID;
-      }
+      m.chroma_mode = (uint8_t)r.ue();
+      if (!intra_modes_ok(c, m, ax.avail)) return PARSE_INVALID;
     }
     if (cbp < 0) {
       cbp = cbp_from_code((int)r.ue(), m.mb_type == MBT_I4x4);
@@ -1131,20 +1081,19 @@ int parse_slice(BitReader& r, const Nal& nal, ParserState* st, ParsedPicture* pi
     }
     m.cbp = (uint8_t)cbp;
     const int cbp_l = cbp & 15, cbp_c = cbp >> 4;
-    if (!intra && cbp_l > 0 && st->transform_8x8 && no_sub8 && r.bit()) ax.flags |= DECAUX_T8;   // transform_size_8x8_flag
+    if (!intra && cbp_l > 0 && c.st->transform_8x8 && no_sub8 && r.bit()) ax.flags |= DECAUX_T8;   // transform_size_8x8_flag
     const bool t8 = (ax.flags & DECAUX_T8) != 0;
     if (cbp > 0 || m.mb_type == MBT_I16x16) {
       const int dqp = r.se();
       if (dqp < -26 || dqp > 25) return PARSE_INVALID;
       qp = (qp + dqp + 52) % 52;                              // 7.4.5: QP_Y wraps modulo 52
-      const int8_t* L = avL ? pic->mbs[idx - 1].nnz : nullptr;
-      const int8_t* T = avT ? pic->mbs[idx - mbw].nnz : nullptr;
+      const int8_t* L = (ax.avail & 1) ? pic->mbs[idx - 1].nnz : nullptr;
+      const int8_t* T = (ax.avail & 2) ? pic->mbs[idx - mbw].nnz : nullptr;
       auto luma_nc = [&](int bx, int by) {
         const int a = bx > 0 ? m.nnz[by * 4 + bx - 1] : (L ? L[by * 4 + 3] : -1);
         const int b = by > 0 ? m.nnz[(by - 1) * 4 + bx] : (T ? T[12 + bx] : -1);
         return nc_of(a, b);
       };
-      int rc;
       if (m.mb_type == MBT_I16x16 && (rc = read_block(r, m.luma_dc, 16, luma_nc(0, 0))) < 0) return rc;
       for (int k = 0; k < 16; k++) {
         if (!(cbp_l & (1 << (k >> 2)))) continue;
@@ -1179,18 +1128,117 @@ int parse_slice(BitReader& r, const Nal& nal, ParserState* st, ParsedPicture* pi
     }
     m.qp = (uint8_t)qp;
     if (!r.ok()) return PARSE_TRUNCATED;
-    track_mb(idx, cur_ri);
+    track_mb(c, idx, ri);
     idx++;
     if (!r.more_data()) break;                                // end of this slice
   }
   pic->next_mb = idx;
-  return track_fail ? PARSE_INVALID : PARSE_OK;
+  return PARSE_OK;
+}
+
+int parse_slice(BitReader& r, const Nal& nal, ParserState* st, ParsedPicture* pic) {
+  SliceCtx c;
+  c.st = st; c.pic = pic;
+  int rc = parse_slice_header(r, nal, st, pic, c);
+  if (rc != PARSE_OK) return rc;
+  if (pic->n_slices == 0) {
+    if ((rc = start_picture(st, pic, c)) != PARSE_OK) return rc;
+  } else if (c.idr != pic->ss.idr || c.ss.frame_num != pic->ss.frame_num || c.is_ref != pic->is_ref || c.poc != pic->poc) {
+    return PARSE_INVALID;                                     // slices of one access unit must agree
+  }
+  c.mbw = st->sp.mb_w; c.n_mb = st->sp.mb_w * st->sp.mb_h;
+  if ((c.is_b || c.wp.on) && !pic->has_b) {                   // B macroblocks, and P macroblocks with explicit weights, travel resolved
+    pic->has_b = true;
+    DecMbAuxB zb;
+    memset(&zb, 0, sizeof(zb));
+    pic->aux_b.assign(c.n_mb, zb);
+  }
+  c.track = !st->motion.empty();
+  if (c.track) { c.M.cur = &st->motion[pic->cur_slot]; c.M.mbw = c.mbw; }
+  if (c.is_b) {
+    BSliceCtx& b = c.b;
+    b.cur_poc = c.poc; b.n_ref[0] = c.n_ref[0]; b.n_ref[1] = c.n_ref[1];
+    for (int l = 0; l < 2; l++) for (int i = 0; i < 33; i++) b.list[l][i] = c.lists[l][i];
+    b.implicit = st->weighted_bipred_idc == 2;
+    b.wp = c.wp.on ? &c.wp : nullptr;
+    b.cabac = st->entropy_cabac;
+    const int cslot = c.lists[1][0].slot;
+    b.col = (cslot >= 0 && cslot < (int)st->motion.size()) ? &st->motion[cslot] : nullptr;
+    b.col_long_term = c.lists[1][0].lt;
+  }
+  if (pic->n_slices >= 65535) return PARSE_UNSUPPORTED;
+  c.slice_no = pic->n_slices++;
+  if (c.dbk_idc != 1) pic->any_deblock = true;
+  rc = st->entropy_cabac ? parse_slice_data_cabac(r, nal, c) : parse_slice_data_cavlc(r, c);
+  if (rc != PARSE_OK) return rc;
+  return c.track_fail ? PARSE_INVALID : PARSE_OK;
+}
+
+// decoded reference picture marking (8.2.5) of a complete reference picture: an IDR picture empties the buffer; otherwise the
+// memory management commands or the sliding window make room, then the picture joins the references (short-term unless a
+// command says otherwise)
+void mark_reference_picture(ParserState* st, const ParsedPicture& pic) {
+  const int max_fn = 1 << st->log2_max_frame_num, cur = pic.ss.frame_num;
+  std::vector<ParserState::RefPic>& refs = st->refs;
+  auto pic_num = [&](const ParserState::RefPic& rp) { return rp.frame_num > cur ? rp.frame_num - max_fn : rp.frame_num; };
+  auto find = [&](bool lt, int num) -> int {                  // the first short-term picture with PicNum num, or long-term one with
+    for (size_t i = 0; i < refs.size(); i++)                  // LongTermFrameIdx num; -1 if none
+      if (refs[i].long_term == lt && (lt ? refs[i].lt_idx : pic_num(refs[i])) == num) return (int)i;
+    return -1;
+  };
+  auto drop_long_term = [&](int lt_idx) { const int j = find(true, lt_idx); if (j >= 0) refs.erase(refs.begin() + j); return j; };
+  bool cur_long = false, reset = false;
+  int cur_lt_idx = 0;
+  if (pic.ss.idr) {
+    refs.clear();
+    cur_long = pic.idr_long_term;
+  } else if (pic.adaptive_marking) {
+    for (const ParsedPicture::Mmco& m : pic.mmco) {
+      if (m.op == 1 || m.op == 3) {                           // a short-term picture: unused, or turned into a long-term one
+        int i = find(false, cur - (m.a + 1));
+        if (i < 0) continue;
+        if (m.op == 1) { refs.erase(refs.begin() + i); continue; }
+        if (const int j = drop_long_term(m.b); j >= 0 && j < i) i--;   // the index is taken over
+        refs[i].long_term = true; refs[i].lt_idx = m.b;
+      } else if (m.op == 2) {
+        drop_long_term(m.a);
+      } else if (m.op == 4) {
+        for (size_t i = 0; i < refs.size();)
+          if (refs[i].long_term && refs[i].lt_idx >= m.a) refs.erase(refs.begin() + i); else i++;
+      } else if (m.op == 5) {
+        refs.clear(); reset = true;
+      } else if (m.op == 6) {
+        drop_long_term(m.b);
+        cur_long = true; cur_lt_idx = m.b;
+      }
+    }
+  }
+  const int cap = st->sp.num_ref_frames < 1 ? 1 : st->sp.num_ref_frames;
+  while ((int)refs.size() >= cap) {                           // sliding window (8.2.5.3): the short-term picture with the smallest FrameNumWrap goes
+    size_t victim = refs.size();
+    int best = 0x7fffffff;
+    for (size_t i = 0; i < refs.size(); i++)
+      if (!refs[i].long_term && pic_num(refs[i]) < best) { best = pic_num(refs[i]); victim = i; }
+    if (victim == refs.size()) victim = 0;                    // only long-term pictures left: a non-conforming stream; drop the first
+    refs.erase(refs.begin() + victim);
+  }
+  ParserState::RefPic rp;
+  rp.slot = pic.cur_slot; rp.frame_num = reset ? 0 : cur; rp.long_term = cur_long; rp.lt_idx = cur_lt_idx;
+  rp.poc = pic.poc; rp.pic_id = pic.pic_id;
+  refs.push_back(rp);
+  st->have_ref = true; st->last_frame_num = reset ? 0 : cur;
+  st->prev_poc_msb = reset ? 0 : pic.poc_msb; st->prev_poc_lsb = reset ? 0 : pic.poc_lsb;
 }
 
 }  // namespace
 
 int parse_access_unit(const uint8_t* au, size_t len, ParserState* st, ParsedPicture* pic) {
   if (!au || !st || !pic) return PARSE_INVALID;
+  {                                                           // a fresh picture that keeps the storage of the record arrays
+    ParsedPicture fresh{};
+    fresh.mbs.swap(pic->mbs); fresh.aux.swap(pic->aux); fresh.aux_b.swap(pic->aux_b); fresh.cabac_info.swap(pic->cabac_info);
+    *pic = std::move(fresh);
+  }
   bool got_slice = false;
   for (const Nal& nal : split_nals(au, len)) {
     BitReader r(nal.rbsp.data(), nal.rbsp.size());
@@ -1207,61 +1255,7 @@ int parse_access_unit(const uint8_t* au, size_t len, ParserState* st, ParsedPict
   }
   if (!got_slice) return PARSE_NO_PICTURE;
   if (pic->next_mb != st->sp.mb_w * st->sp.mb_h) return PARSE_INCOMPLETE;    // macroblocks missing: more slices to come (or lost: needs concealment)
-  if (pic->is_ref) {
-    // decoded reference picture marking (8.2.5): an IDR picture empties the buffer; otherwise the memory management commands
-    // or the sliding window make room, then the picture joins the references (short-term unless a command says otherwise)
-    const int max_fn = 1 << st->log2_max_frame_num, cur = pic->ss.frame_num;
-    auto pic_num = [&](const ParserState::RefPic& rp) { return rp.frame_num > cur ? rp.frame_num - max_fn : rp.frame_num; };
-    bool cur_long = false, reset = false;
-    int cur_lt_idx = 0;
-    if (pic->ss.idr) {
-      st->refs.clear();
-      if (pic->idr_long_term) { cur_long = true; cur_lt_idx = 0; }
-    } else if (pic->adaptive_marking) {
-      for (const ParsedPicture::Mmco& m : pic->mmco) {
-        if (m.op == 1 || m.op == 3) {                           // a short-term picture: unused, or turned into a long-term one
-          const int want = cur - (m.a + 1);
-          for (size_t i = 0; i < st->refs.size(); i++) {
-            if (st->refs[i].long_term || pic_num(st->refs[i]) != want) continue;
-            if (m.op == 1) st->refs.erase(st->refs.begin() + i);
-            else {
-              for (size_t j = 0; j < st->refs.size(); j++)      // the index is taken over
-                if (st->refs[j].long_term && st->refs[j].lt_idx == m.b && j != i) { st->refs.erase(st->refs.begin() + j); if (j < i) i--; break; }
-              st->refs[i].long_term = true; st->refs[i].lt_idx = m.b;
-            }
-            break;
-          }
-        } else if (m.op == 2) {
-          for (size_t i = 0; i < st->refs.size(); i++)
-            if (st->refs[i].long_term && st->refs[i].lt_idx == m.a) { st->refs.erase(st->refs.begin() + i); break; }
-        } else if (m.op == 4) {
-          for (size_t i = 0; i < st->refs.size();)
-            if (st->refs[i].long_term && st->refs[i].lt_idx >= m.a) st->refs.erase(st->refs.begin() + i); else i++;
-        } else if (m.op == 5) {
-          st->refs.clear(); reset = true;
-        } else if (m.op == 6) {
-          for (size_t j = 0; j < st->refs.size(); j++)
-            if (st->refs[j].long_term && st->refs[j].lt_idx == m.b) { st->refs.erase(st->refs.begin() + j); break; }
-          cur_long = true; cur_lt_idx = m.b;
-        }
-      }
-    }
-    const int cap = st->sp.num_ref_frames < 1 ? 1 : st->sp.num_ref_frames;
-    while ((int)st->refs.size() >= cap) {                      // sliding window (8.2.5.3): the short-term picture with the smallest FrameNumWrap goes
-      size_t victim = st->refs.size();
-      int best = 0x7fffffff;
-      for (size_t i = 0; i < st->refs.size(); i++)
-        if (!st->refs[i].long_term && pic_num(st->refs[i]) < best) { best = pic_num(st->refs[i]); victim = i; }
-      if (victim == st->refs.size()) victim = 0;               // only long-term pictures left: a non-conforming stream; drop the first
-      st->refs.erase(st->refs.begin() + victim);
-    }
-    ParserState::RefPic rp;
-    rp.slot = pic->cur_slot; rp.frame_num = reset ? 0 : cur; rp.long_term = cur_long; rp.lt_idx = cur_lt_idx;
-    rp.poc = pic->poc; rp.pic_id = pic->pic_id;
-    st->refs.push_back(rp);
-    st->have_ref = true; st->last_frame_num = reset ? 0 : cur;
-    st->prev_poc_msb = reset ? 0 : pic->poc_msb; st->prev_poc_lsb = reset ? 0 : pic->poc_lsb;
-  }
+  if (pic->is_ref) mark_reference_picture(st, *pic);
   st->decode_count = pic->ss.idr ? 1 : st->decode_count + 1;
   return PARSE_OK;
 }

@@ -106,7 +106,6 @@ struct ParserState {
 
 struct ParsedPicture {
   SliceState ss;                 // idr, frame_num, idr_pic_id, slice qp
-  int disable_deblocking_idc = 0;
   bool is_ref = true;            // nal_ref_idc != 0
   int crop_left = 0, crop_top = 0;   // luma samples to drop at the left / top of the decoded picture
   std::vector<MbOut> mbs;        // mb_w * mb_h records, same meaning as the encoder's hand-over records
@@ -128,12 +127,12 @@ struct ParsedPicture {
   struct Mmco { int op, a, b; };  // memory_management_control_operation with its operands
   std::vector<Mmco> mmco;
   bool idr_long_term = false;    // long_term_reference_flag of an IDR picture
-  std::vector<int> mmco1_diff_unused;   // difference_of_pic_nums_minus1 of each "mark short-term picture unused" command
   bool any_deblock = false;      // some slice wants its macroblocks filtered
   std::vector<CabacMbInfo> cabac_info;   // scratch of the CABAC slice-data parser (one per macroblock)
 };
 
-// Parses one access unit: [SPS] [PPS] slice, each NAL behind a 3- or 4-byte start code.  Returns PARSE_OK or an error.
+// Parses one access unit: [SPS] [PPS] slice, each NAL behind a 3- or 4-byte start code, into a fresh *pic (whose record arrays keep
+// their storage).  Returns PARSE_OK or an error.
 int parse_access_unit(const uint8_t* au, size_t len, ParserState* st, ParsedPicture* pic);
 // without state: is there a slice, and the cropped size of the SPS the unit carries (0 x 0 if none)
 int probe_access_unit(const uint8_t* au, size_t len, int* width, int* height, int* has_slice);

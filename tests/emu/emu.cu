@@ -118,7 +118,6 @@ struct HostFrameEncoder {
       double us = 0;
       for (int r = 0; r < g_emu_time_writer; r++) {
         b2h264::ParserState ps = parser;
-        tp.next_mb = 0; tp.n_slices = 0;
         const auto t0 = std::chrono::steady_clock::now();
         b2h264::parse_access_unit(au.data(), au.size(), &ps, &tp);
         us += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
