@@ -2,20 +2,12 @@
 #include "broker.h"
 
 #include <cuda_runtime_api.h>
-#include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 namespace b2wels {
 
-static long env_long(const char* name, long dflt) {
-  const char* v = getenv(name);
-  return v && *v ? atol(v) : dflt;
-}
-
-Pool::Pool(const PoolKey& key, int capacity, int device) : key_(key), cap_(capacity), device_(device) {
+EncPool::EncPool(const PoolKey& key, int capacity, int device) : Batcher(capacity), key_(key), device_(device) {
   frame_bytes_ = (size_t)key.width * key.height * 3 / 2;
-  wait_us_ = env_long("B2H264_BROKER_WAIT_US", 2000);
   b2h264_enc_config cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.width = key.width; cfg.height = key.height; cfg.qp = key.qp; cfg.fps = key.fps;
@@ -44,110 +36,58 @@ Pool::Pool(const PoolKey& key, int capacity, int device) : key_(key), cap_(capac
     return;
   }
   up_stream_ = us;
-  state_.assign(capacity, FREE);
   au_.resize(capacity);
   idr_.assign(capacity, 0);
 }
 
-Pool::~Pool() {
+EncPool::~EncPool() {
   if (enc_) b2h264_enc_destroy(enc_);
   if (pinned_) cudaFreeHost(pinned_);
   if (d_stage_) { cudaSetDevice(device_); cudaFree(d_stage_); }
   if (up_stream_) cudaStreamDestroy((cudaStream_t)up_stream_);
 }
 
-int Pool::upload(int slot) {
+int EncPool::upload(int slot) {
   if (cudaSetDevice(device_) != cudaSuccess) return -1;
   return cudaMemcpyAsync(d_stage_ + (size_t)slot * frame_bytes_, pinned_ + (size_t)slot * frame_bytes_, frame_bytes_, cudaMemcpyHostToDevice,
                          (cudaStream_t)up_stream_) == cudaSuccess ? 0 : -1;
 }
 
-int Pool::acquire() {
-  std::unique_lock<std::mutex> lk(m_);
-  for (int s = 0; s < cap_; s++)
-    if (state_[s] == FREE) { state_[s] = IDLE; n_registered_++; return s; }
-  return -1;
+int EncPool::force_idr(int slot) {
+  return when_idle([&] { return b2h264_enc_force_idr(enc_, slot); });
 }
 
-void Pool::release(int slot) {
-  std::unique_lock<std::mutex> lk(m_);
-  cv_.wait(lk, [&] { return !flushing_; });            // nothing of this pool is in flight now
-  b2h264_enc_reset_stream(enc_, slot);
-  state_[slot] = FREE;
-  n_registered_--;
-  cv_.notify_all();                                    // "everybody is waiting" may have become true
-}
-
-int Pool::registered() {
-  std::unique_lock<std::mutex> lk(m_);
-  return n_registered_;
-}
-
-int Pool::force_idr(int slot) {
-  std::unique_lock<std::mutex> lk(m_);
-  cv_.wait(lk, [&] { return !flushing_; });
-  return b2h264_enc_force_idr(enc_, slot);
-}
-
-// codes every PENDING picture as one batch; called with the lock held, returns with it held
-void Pool::flush_locked(std::unique_lock<std::mutex>& lk) {
-  flushing_ = true;
-  std::vector<const uint8_t*> src(cap_, nullptr);
-  for (int s = 0; s < cap_; s++)
-    if (state_[s] == PENDING) { state_[s] = INFLIGHT; src[s] = d_stage_ + (size_t)s * frame_bytes_; }
-  n_pending_ = 0;
-  lk.unlock();
-  std::vector<const uint8_t*> bs(cap_, nullptr);
+void EncPool::code_batch(const std::vector<int>& slots, int* result) {
+  std::vector<const uint8_t*> src(cap_, nullptr), bs(cap_, nullptr);
   std::vector<int32_t> nb(cap_, 0), ft(cap_, 0);
-  // every pending stream enqueued its upload before it registered as pending: one wait covers them all
+  for (int s : slots) src[s] = d_stage_ + (size_t)s * frame_bytes_;
+  // every stream of the batch enqueued its upload before it joined: one wait covers them all
   int rc = cudaSetDevice(device_) == cudaSuccess && cudaStreamSynchronize((cudaStream_t)up_stream_) == cudaSuccess ? 0 : -1;
   if (rc == 0) rc = b2h264_enc_submit(enc_, src.data(), 1);
   if (rc == 0) rc = b2h264_enc_collect(enc_, bs.data(), nb.data(), ft.data());
-  lk.lock();
-  for (int s = 0; s < cap_; s++) {
-    if (state_[s] != INFLIGHT) continue;
-    if (rc == 0 && bs[s]) { au_[s].assign(bs[s], bs[s] + nb[s]); idr_[s] = ft[s] == 1; state_[s] = DONE; }
-    else state_[s] = FAILED;
+  for (int s : slots) {
+    if (rc == 0 && bs[s]) { au_[s].assign(bs[s], bs[s] + nb[s]); idr_[s] = ft[s] == 1; }
+    result[s] = rc ? rc : (bs[s] ? 0 : -1);
   }
-  last_rc_ = rc;
-  flushing_ = false;
-  cv_.notify_all();
 }
 
-int Pool::encode(int slot, std::vector<uint8_t>* au, bool* idr) {
-  std::unique_lock<std::mutex> lk(m_);
-  if (slot < 0 || slot >= cap_ || state_[slot] != IDLE) return -1;
-  state_[slot] = PENDING;
-  n_pending_++;
-  const auto deadline = std::chrono::steady_clock::now() + std::chrono::microseconds(wait_us_);
-  while (state_[slot] != DONE && state_[slot] != FAILED) {
-    if (state_[slot] == PENDING && !flushing_) {
-      if (n_pending_ >= n_registered_ || std::chrono::steady_clock::now() >= deadline) { flush_locked(lk); continue; }
-      cv_.wait_until(lk, deadline);
-    } else {
-      cv_.wait(lk);
-    }
-  }
-  const bool ok = state_[slot] == DONE;
-  if (ok) { au->swap(au_[slot]); *idr = idr_[slot] != 0; }
-  state_[slot] = IDLE;
-  return ok ? 0 : (last_rc_ ? last_rc_ : -1);
+int EncPool::encode(int slot, std::vector<uint8_t>* au, bool* idr) {
+  const int rc = run(slot);
+  if (rc == 0) { au->swap(au_[slot]); *idr = idr_[slot] != 0; }
+  return rc;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-DecPool::DecPool(int width, int height, int capacity, int device) : w_(width), h_(height), cap_(capacity), device_(device) {
+DecPool::DecPool(int width, int height, int capacity, int device) : Batcher(capacity), w_(width), h_(height) {
   frame_bytes_ = (size_t)width * height * 3 / 2;
-  wait_us_ = env_long("B2H264_BROKER_WAIT_US", 2000);
   b2h264_dec_config cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.width = width; cfg.height = height; cfg.n_streams = capacity; cfg.device = device;
   if (b2h264_dec_create(&cfg, &dec_) != 0) { dec_ = nullptr; return; }
   pinned_ = static_cast<uint8_t*>(b2h264_host_alloc(frame_bytes_ * capacity));
   if (!pinned_) { b2h264_dec_destroy(dec_); dec_ = nullptr; return; }
-  state_.assign(capacity, FREE);
   au_.assign(capacity, nullptr);
   bytes_.assign(capacity, 0);
-  status_.assign(capacity, 0);
 }
 
 DecPool::~DecPool() {
@@ -155,67 +95,20 @@ DecPool::~DecPool() {
   if (pinned_) b2h264_host_free(pinned_);
 }
 
-int DecPool::acquire() {
-  std::unique_lock<std::mutex> lk(m_);
-  for (int s = 0; s < cap_; s++)
-    if (state_[s] == FREE) { state_[s] = IDLE; n_registered_++; return s; }
-  return -1;
-}
-
-void DecPool::release(int slot) {
-  std::unique_lock<std::mutex> lk(m_);
-  cv_.wait(lk, [&] { return !flushing_; });
-  b2h264_dec_reset_stream(dec_, slot);
-  state_[slot] = FREE;
-  n_registered_--;
-  cv_.notify_all();
-}
-
-int DecPool::registered() {
-  std::unique_lock<std::mutex> lk(m_);
-  return n_registered_;
-}
-
-void DecPool::flush_locked(std::unique_lock<std::mutex>& lk) {
-  flushing_ = true;
+void DecPool::code_batch(const std::vector<int>& slots, int* result) {
   std::vector<const uint8_t*> au(cap_, nullptr);
   std::vector<int32_t> nb(cap_, 0), st(cap_, 0);
-  std::vector<uint8_t*> out(cap_, nullptr);
-  for (int s = 0; s < cap_; s++) {
-    out[s] = pinned_ + (size_t)s * frame_bytes_;
-    if (state_[s] == PENDING) { state_[s] = INFLIGHT; au[s] = au_[s]; nb[s] = bytes_[s]; }
-  }
-  n_pending_ = 0;
-  lk.unlock();
+  std::vector<uint8_t*> out(cap_);
+  for (int s = 0; s < cap_; s++) out[s] = picture(s);
+  for (int s : slots) { au[s] = au_[s]; nb[s] = bytes_[s]; }
   const int rc = b2h264_dec_decode3(dec_, au.data(), nb.data(), out.data(), st.data());
-  lk.lock();
-  for (int s = 0; s < cap_; s++) {
-    if (state_[s] != INFLIGHT) continue;
-    status_[s] = rc ? (rc > 0 ? -1000 - rc : rc) : st[s];        // a failure of the call as a whole fails every stream of the batch
-    state_[s] = DONE;
-  }
-  flushing_ = false;
-  cv_.notify_all();
+  for (int s : slots) result[s] = rc ? (rc > 0 ? -1000 - rc : rc) : st[s];   // a failure of the call as a whole fails every stream of the batch
 }
 
 int DecPool::decode(int slot, const uint8_t* au, int32_t bytes) {
-  std::unique_lock<std::mutex> lk(m_);
-  if (slot < 0 || slot >= cap_ || state_[slot] != IDLE) return -1;
+  if (slot < 0 || slot >= cap_) return -1;
   au_[slot] = au; bytes_[slot] = bytes;
-  state_[slot] = PENDING;
-  n_pending_++;
-  const auto deadline = std::chrono::steady_clock::now() + std::chrono::microseconds(wait_us_);
-  while (state_[slot] != DONE) {
-    if (state_[slot] == PENDING && !flushing_) {
-      if (n_pending_ >= n_registered_ || std::chrono::steady_clock::now() >= deadline) { flush_locked(lk); continue; }
-      cv_.wait_until(lk, deadline);
-    } else {
-      cv_.wait(lk);
-    }
-  }
-  const int st = status_[slot];
-  state_[slot] = IDLE;
-  return st;
+  return run(slot);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -224,66 +117,42 @@ Broker& Broker::get() {
   return *b;
 }
 
-std::shared_ptr<Pool> Broker::attach(const PoolKey& key, int* slot) {
+template <class P, class... Args>
+std::shared_ptr<P> Broker::attach_pool(int* slot, const Args&... args) {
   std::lock_guard<std::mutex> g(m_);
   int same_class = 0;
-  for (auto& p : pools_) {
-    if (!(p->key() == key)) continue;
+  for (auto& b : pools_) {
+    auto p = std::dynamic_pointer_cast<P>(b);
+    if (!p || !p->serves(args...)) continue;
     same_class++;
     const int s = p->acquire();
     if (s >= 0) { *slot = s; return p; }
   }
-  // capacity: B2H264_BROKER_SLOTS, else 4, 16, 64, 128, 128, ... for successive pools of a class (a lone encoder stays
-  // small: a slot costs ~30 MB of HBM and ~25 MB of pinned host memory at 1080p)
+  // capacity: B2H264_BROKER_SLOTS, else 4, 16, 64, 128, 128, ... for successive pools of a class (a lone stream stays
+  // small: an encoder slot costs ~30 MB of HBM and ~25 MB of pinned host memory at 1080p)
   long cap = env_long("B2H264_BROKER_SLOTS", 0);
   if (cap <= 0) { cap = 4L << (2 * (same_class < 3 ? same_class : 3)); if (cap > 128) cap = 128; }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) return nullptr;
   const long dev_env = env_long("B2H264_DEVICE", -1);
   const int device = dev_env >= 0 ? (int)(dev_env % ndev) : (next_device_++ % ndev);
-  auto p = std::make_shared<Pool>(key, (int)cap, device);
+  auto p = std::make_shared<P>(args..., (int)cap, device);
   if (!p->ok()) return nullptr;
   pools_.push_back(p);
   *slot = p->acquire();
   return p;
 }
 
-std::shared_ptr<DecPool> Broker::attach_decoder(int width, int height, int* slot) {
-  std::lock_guard<std::mutex> g(m_);
-  int same_class = 0;
-  for (auto& p : dec_pools_) {
-    if (p->width() != width || p->height() != height) continue;
-    same_class++;
-    const int s = p->acquire();
-    if (s >= 0) { *slot = s; return p; }
-  }
-  long cap = env_long("B2H264_BROKER_SLOTS", 0);
-  if (cap <= 0) { cap = 4L << (2 * (same_class < 3 ? same_class : 3)); if (cap > 128) cap = 128; }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) return nullptr;
-  const long dev_env = env_long("B2H264_DEVICE", -1);
-  const int device = dev_env >= 0 ? (int)(dev_env % ndev) : (next_device_++ % ndev);
-  auto p = std::make_shared<DecPool>(width, height, (int)cap, device);
-  if (!p->ok()) return nullptr;
-  dec_pools_.push_back(p);
-  *slot = p->acquire();
-  return p;
-}
+std::shared_ptr<EncPool> Broker::attach(const PoolKey& key, int* slot) { return attach_pool<EncPool>(slot, key); }
 
-void Broker::detach_decoder(const std::shared_ptr<DecPool>& pool, int slot) {
-  pool->release(slot);
-  std::lock_guard<std::mutex> g(m_);
-  if (pool->registered() == 0)
-    for (size_t i = 0; i < dec_pools_.size(); i++)
-      if (dec_pools_[i] == pool) { dec_pools_.erase(dec_pools_.begin() + i); break; }
-}
+std::shared_ptr<DecPool> Broker::attach_decoder(int width, int height, int* slot) { return attach_pool<DecPool>(slot, width, height); }
 
-void Broker::detach(const std::shared_ptr<Pool>& pool, int slot) {
+void Broker::detach(const std::shared_ptr<Batcher>& pool, int slot) {
   pool->release(slot);
   std::lock_guard<std::mutex> g(m_);
   if (pool->registered() == 0)
     for (size_t i = 0; i < pools_.size(); i++)
-      if (pools_[i] == pool) { pools_.erase(pools_.begin() + i); break; }     // the last reference frees the encoder
+      if (pools_[i] == pool) { pools_.erase(pools_.begin() + i); break; }     // the last reference frees the coder
 }
 
 }  // namespace b2wels

@@ -230,7 +230,7 @@ class B2Decoder : public ISVCDecoder {
   bool inited_ = false, eos_ = false;
   int ec_ = 0, vcl_ = 0;
   void drop_slot() {
-    if (pool_) { b2wels::Broker::get().detach_decoder(pool_, slot_); pool_.reset(); }
+    if (pool_) { b2wels::Broker::get().detach(pool_, slot_); pool_.reset(); }
     slot_ = -1; pic_ = nullptr;
     held_.clear(); has_b_ = have_out_ = false; seq_ = last_out_seq_ = last_out_poc_ = 0;
   }

@@ -274,7 +274,7 @@ class B2Encoder : public ISVCEncoder {
     info->uiTimeStamp = ts;
   }
 
-  std::shared_ptr<b2wels::Pool> pool_;
+  std::shared_ptr<b2wels::EncPool> pool_;
   int slot_ = -1;
   SEncParamExt par_;
   int w_ = 0, h_ = 0;
