@@ -69,14 +69,37 @@ int  b2h264_enc_submit (b2h264_enc* e, const uint8_t* const* src, int src_on_dev
 
 /* Waits for the oldest submitted batch, entropy-codes it, and returns per-stream Annex-B access units.
  * bs[i] / bs_bytes[i]: encoder-owned buffer of stream i, valid until the next collect on this encoder
- * (like SFrameBSInfo::pBsBuf, codec_app_def.h:647-654).  frame_type[i]: 1 = IDR, 2 = P (may be NULL). */
+ * (like SFrameBSInfo::pBsBuf, codec_app_def.h:647-654).  frame_type[i]: 1 = IDR, 2 = P, 0 = the stream sat
+ * the call out, -1 = its picture was not coded (bs[i] NULL: a recovery request found no confirmed long-term picture, and the
+ * stream's next picture is an IDR; the reference's EncodeFrame fails the same way) (may be NULL). */
 int  b2h264_enc_collect (b2h264_enc* e, const uint8_t** bs, int32_t* bs_bytes, int32_t* frame_type);
 
 /* next picture of stream i (or all streams when i < 0) is coded as IDR (ISVCEncoder::ForceIntraFrame) */
 int  b2h264_enc_force_idr (b2h264_enc* e, int stream);
 
+/* Reference pictures, before the first submit (-3 after it; -2 for a value out of range).  num_ref_frames is
+ * SEncParamExt::iNumRefFrame: -1 (AUTO_REF_PIC_COUNT) or 1..10; with ltr_enable (bEnableLongTermReference) the encoder keeps
+ * two long-term pictures and marks a new one every ltr_mark_period (iLtrMarkPeriod) P pictures once the last is confirmed.
+ * Resolved as the reference resolves them: max_num_ref_frames of the SPS is the larger of num_ref_frames and what LTR needs
+ * (1, or 3 with LTR).  Each stream keeps 2 pictures on the device without LTR and 4 with it.  Defaults: 1, 0, 30.
+ * b2h264_enc_get_references: out4 = iNumRefFrame and max_num_ref_frames as resolved, iLTRRefNum, pictures kept per stream. */
+int  b2h264_enc_set_references (b2h264_enc* e, int num_ref_frames, int ltr_enable, int ltr_mark_period);
+int  b2h264_enc_get_references (b2h264_enc* e, int32_t* out4);
+
+/* Loss-recovery feedback of stream i (SLTRRecoverRequest / SLTRMarkingFeedback of ENCODER_LTR_RECOVERY_REQUEST /
+ * ENCODER_LTR_MARKING_FEEDBACK; feedback_type 1 = LTR_RECOVERY_REQUEST, 4 / 5 = LTR_MARKING_SUCCESS / _FAILED).  It takes
+ * effect on the stream's next submitted picture: a valid recovery request makes it predict from the newest confirmed
+ * long-term picture, a request with last_correct_frame_num -1 (or any request while LTR is off) makes it an IDR; a valid request while no long-term
+ * picture is confirmed drops the next picture (b2h264_enc_collect: frame type -1) and makes the one after it an IDR.  Feedback
+ * whose idr_pic_id is not that of the stream's last IDR is ignored.  b2h264_enc_ltr_mark_period changes the marking period
+ * of one stream (ENCODER_LTR_MARKING_PERIOD). */
+int  b2h264_enc_ltr_recovery_request (b2h264_enc* e, int stream, int feedback_type, int idr_pic_id, int cur_frame_num,
+                                      int last_correct_frame_num);
+int  b2h264_enc_ltr_marking_feedback (b2h264_enc* e, int stream, int feedback_type, int idr_pic_id, int ltr_frame_num);
+int  b2h264_enc_ltr_mark_period (b2h264_enc* e, int stream, int period);
+
 /* stream i starts over as a fresh encoder would (next picture IDR, parameter-set ids, frame_num, SAD / reference
- * history cleared); only while nothing is in flight.  Used when an ISVCEncoder slot of a shared encoder is re-used. */
+ * history and long-term state cleared); only while nothing is in flight.  Used when an ISVCEncoder slot of a shared encoder is re-used. */
 int  b2h264_enc_reset_stream (b2h264_enc* e, int stream);
 
 /* Exact CAVLC bit count on the device (the reference's rate control reads it from the bitstream position per macroblock:
@@ -87,7 +110,7 @@ int  b2h264_enc_reset_stream (b2h264_enc* e, int stream);
 int  b2h264_enc_set_mb_bits (b2h264_enc* e, int on);
 int  b2h264_enc_get_mb_bits (b2h264_enc* e, int stream, int32_t* device_bits, int32_t* host_bits);
 
-/* copies the reconstructed (deblocked) picture of stream i that is currently the reference into dst
+/* copies the picture of stream i reconstructed (and deblocked) last into dst
  * (cropped I420, w*h*3/2 bytes, host memory): for parity tests */
 int  b2h264_enc_get_recon (b2h264_enc* e, int stream, uint8_t* h_dst);
 

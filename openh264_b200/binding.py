@@ -83,6 +83,11 @@ API = {
     "b2h264_enc_set_mb_bits": [vp, C.c_int],
     "b2h264_enc_get_mb_bits": [vp, C.c_int, i32p, i32p],
     "b2h264_enc_get_recon": [vp, C.c_int, vp],
+    "b2h264_enc_set_references": [vp, C.c_int, C.c_int, C.c_int],
+    "b2h264_enc_get_references": [vp, i32p],
+    "b2h264_enc_ltr_recovery_request": [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int],
+    "b2h264_enc_ltr_marking_feedback": [vp, C.c_int, C.c_int, C.c_int, C.c_int],
+    "b2h264_enc_ltr_mark_period": [vp, C.c_int, C.c_int],
     "b2h264_enc_last_timing": [vp, C.POINTER(C.c_float)],
     "b2h264_enc_last_d2h_bytes": [vp, C.POINTER(C.c_ulonglong)],
     "b2h264_enc_last_coded_mbs": [vp, C.POINTER(C.c_ulonglong)],
@@ -198,7 +203,10 @@ class BatchEncoder:
     stream per call; returns the Annex-B access units.  No computation happens in Python."""
 
     def __init__(self, width, height, qp=26, fps=30.0, n_streams=1, target_bitrate=5000000, entropy_threads=0, device=0,
-                 sps_pps_id_strategy=1, complexity_low=False, entropy_cabac=False, profile_idc=0, intra_period=0, loop_filter=(0, 0, 0)):
+                 sps_pps_id_strategy=1, complexity_low=False, entropy_cabac=False, profile_idc=0, intra_period=0, loop_filter=(0, 0, 0),
+                 num_ref_frames=1, ltr=False, ltr_mark_period=30):
+        """num_ref_frames (iNumRefFrame: -1 = AUTO_REF_PIC_COUNT, or 1..10), ltr (bEnableLongTermReference) and ltr_mark_period
+        (iLtrMarkPeriod): b2h264_enc_set_references"""
         self.L = lib(device)
         self.cfg = EncConfig(width, height, qp, fps, target_bitrate, n_streams, entropy_threads, device, sps_pps_id_strategy,
                              1 if complexity_low else 0, 1 if entropy_cabac else 0, profile_idc, intra_period, *loop_filter)
@@ -206,6 +214,26 @@ class BatchEncoder:
         check(self.L.b2h264_enc_create(C.byref(self.cfg), C.byref(self.h)))
         self.n = n_streams
         self.frame_bytes = width * height * 3 // 2
+        if (num_ref_frames, bool(ltr), ltr_mark_period) != (1, False, 30):
+            check(self.L.b2h264_enc_set_references(self.h, num_ref_frames, 1 if ltr else 0, ltr_mark_period))
+
+    def references(self):
+        """(iNumRefFrame, max_num_ref_frames, iLTRRefNum, pictures kept per stream) as resolved"""
+        v = (C.c_int32 * 4)()
+        check(self.L.b2h264_enc_get_references(self.h, v))
+        return tuple(v)
+
+    def ltr_recovery_request(self, stream, idr_pic_id, cur_frame_num, last_correct_frame_num, feedback_type=1):
+        """ENCODER_LTR_RECOVERY_REQUEST for one stream (feedback_type 1 = LTR_RECOVERY_REQUEST); applies to its next picture"""
+        check(self.L.b2h264_enc_ltr_recovery_request(self.h, stream, feedback_type, idr_pic_id, cur_frame_num, last_correct_frame_num))
+
+    def ltr_marking_feedback(self, stream, idr_pic_id, ltr_frame_num, success=True):
+        """ENCODER_LTR_MARKING_FEEDBACK for one stream (LTR_MARKING_SUCCESS or LTR_MARKING_FAILED); applies to its next picture"""
+        check(self.L.b2h264_enc_ltr_marking_feedback(self.h, stream, 4 if success else 5, idr_pic_id, ltr_frame_num))
+
+    def ltr_mark_period(self, stream, period):
+        """ENCODER_LTR_MARKING_PERIOD for one stream"""
+        check(self.L.b2h264_enc_ltr_mark_period(self.h, stream, period))
 
     def submit(self, frames, on_device=False):
         """frames: list of n_streams numpy uint8 arrays (host) or raw device pointers (on_device=True)."""

@@ -81,7 +81,8 @@ int pack_records_compact(const MbOut* mbs, int n, uint8_t* dst, int32_t* idx) {
 
 // compact records (enc_kernels.cu: k_pack_records): idx[mb] = offset in 32-byte units or -1; 128-byte head
 // (MbOut bytes [0, 112) + chroma_dc, presence mask of the 24 residual blocks in pad0) + 32 bytes per present block
-void StreamCtl::write_access_unit_packed(bool idr, const MbOut* packed, const int32_t* idx, std::vector<uint8_t>* au) {
+void StreamCtl::write_access_unit_packed(bool idr, const MbOut* packed, const int32_t* idx, std::vector<uint8_t>* au,
+                                         const RefDecision* refs) {
   static const MbOut kSkip = [] { MbOut m; memset(&m, 0, sizeof(m)); m.mb_type = MBT_PSKIP; return m; }();
   const int n = sp.mb_w * sp.mb_h;
   recs_.resize(n);
@@ -106,14 +107,14 @@ void StreamCtl::write_access_unit_packed(bool idr, const MbOut* packed, const in
       if ((mask >> b) & 1) { memcpy(b < 16 ? m.luma[b] : m.chroma_ac[b - 16], blk, 32); blk += 32; }
     recs_[i] = &m;
   }
-  write_au(idr, recs_.data(), au);
+  write_au(idr, recs_.data(), au, refs);
 }
 
-void StreamCtl::write_au(bool idr, const MbOut* const* mbs, std::vector<uint8_t>* au) {
+void StreamCtl::write_au(bool idr, const MbOut* const* mbs, std::vector<uint8_t>* au, const RefDecision* refs) {
   std::vector<uint8_t>& rbsp = rbsp_;             // kept between pictures: its capacity settles at the stream's picture size
   rbsp.clear();
   if (idr) {
-    idr_pic_id = idr_pic_id < 65535 ? idr_pic_id + 1 : 0;
+    idr_pic_id = refs ? refs->idr_pic_id : (idr_pic_id < 65535 ? idr_pic_id + 1 : 0);
     frame_num = 0;
     if (increasing_ids) { sp.sps_id = parasets_written % 32; sp.pps_id = parasets_written % 57; }
     parasets_written++;
@@ -121,7 +122,14 @@ void StreamCtl::write_au(bool idr, const MbOut* const* mbs, std::vector<uint8_t>
     write_pps(sp, &rbsp); append_nal(au, 3, 8, rbsp); rbsp.clear();
   }
   SliceState ss;
+  if (refs) frame_num = refs->frame_num;          // the reference state numbers the pictures it decided (enc_refs.h)
   ss.idr = idr; ss.frame_num = frame_num; ss.idr_pic_id = idr_pic_id; ss.qp = sp.qp;
+  if (refs) {
+    ss.mod_idc = refs->mod_idc; ss.mod_val = refs->mod_val;
+    ss.long_term_reference_flag = refs->long_term_reference_flag;
+    ss.n_mmco = refs->n_mmco;
+    memcpy(ss.mmco, refs->mmco, sizeof(ss.mmco));
+  }
   if (sp.entropy_cabac) write_slice_cabac(sp, ss, mbs, &rbsp);
   else write_slice(sp, ss, mbs, &rbsp, record_mb_bits ? &last_mb_bits : nullptr);
   append_nal(au, 3, idr ? 5 : 1, rbsp);

@@ -7,6 +7,7 @@
 #pragma once
 #include <vector>
 
+#include "enc_refs.h"
 #include "enc_types.h"
 #include "h264_bitstream.h"
 
@@ -21,6 +22,8 @@ int pack_records_compact(const MbOut* mbs, int n, uint8_t* dst, int32_t* idx);
 struct StreamCtl {
   StreamParams sp;
   float fps;
+  // numbering of the picture written last; write_access_unit_packed takes both from the picture's RefDecision (StreamRefs numbers
+  // the pictures), write_access_unit (one-reference host path) counts them here
   int frame_num = 0;
   int idr_pic_id = 0;
   long frames_coded = 0;
@@ -50,10 +53,14 @@ struct StreamCtl {
   EncFrameParams frame_params(bool idr, bool ref_is_p) const;
   // serialises the access unit of the frame just coded (SPS+PPS+IDR slice, or P slice)
   void write_access_unit(bool idr, const MbOut* mbs, std::vector<uint8_t>* au);                 // one record per MB
-  // compact form (k_pack_records): idx[mb] = offset of the macroblock's record in `packed` in 32-byte units, or -1 for P_SKIP
-  void write_access_unit_packed(bool idr, const MbOut* packed, const int32_t* idx, std::vector<uint8_t>* au);
+  // compact form (k_pack_records): idx[mb] = offset of the macroblock's record in `packed` in 32-byte units, or -1 for P_SKIP;
+  // refs: the picture's reference syntax (enc_refs.h), NULL for the one-reference stream's
+  void write_access_unit_packed(bool idr, const MbOut* packed, const int32_t* idx, std::vector<uint8_t>* au,
+                                const RefDecision* refs = nullptr);
+  // max_num_ref_frames of the SPS; the level follows from it (after init)
+  void set_num_ref_frames(int n, int target_bitrate) { sp.num_ref_frames = n; select_level(&sp, fps, target_bitrate); }
  private:
-  void write_au(bool idr, const MbOut* const* recs, std::vector<uint8_t>* au);
+  void write_au(bool idr, const MbOut* const* recs, std::vector<uint8_t>* au, const RefDecision* refs = nullptr);
   std::vector<const MbOut*> recs_;
   std::vector<uint8_t> rbsp_;               // payload of the NAL being written (reused from picture to picture)
   std::vector<MbOut> expand_;               // compact records of the coded macroblocks, expanded for the slice writer

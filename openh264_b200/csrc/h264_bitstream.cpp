@@ -76,7 +76,7 @@ void write_sps(const StreamParams& sp, std::vector<uint8_t>* rbsp) {
   w.ue(15 - 4);                         // log2_max_frame_num_minus4
   w.ue(2);                              // pic_order_cnt_type
   w.ue((uint32_t)sp.num_ref_frames);
-  w.bit(0);                             // gaps_in_frame_num_value_allowed_flag (1 layer, 1 ref)
+  w.bit(sp.num_ref_frames != 1);        // gaps_in_frame_num_value_allowed_flag: set unless one layer has one reference (au_set.cpp:540-544)
   w.ue((uint32_t)sp.mb_w - 1);
   w.ue((uint32_t)sp.mb_h - 1);
   w.bit(1);                             // frame_mbs_only_flag
@@ -187,10 +187,7 @@ inline int nc_of(int a, int b) {          // a/b = neighbour counts or -1 when u
 
 const uint8_t* cbp_me_table(bool intra) { return intra ? kCbpIntra : kCbpInter; }
 
-void write_slice(const StreamParams& sp, const SliceState& ss, const MbOut* const* recs, std::vector<uint8_t>* rbsp,
-                 std::vector<int32_t>* mb_bits) {
-  BitWriter w(rbsp);
-  // ---- slice header (svc_encode_slice.cpp:275-346) ----
+void write_slice_header(BitWriter& w, const StreamParams& sp, const SliceState& ss) {
   w.ue(0);                               // first_mb_in_slice
   w.ue(ss.idr ? 2 : 0);                  // slice_type: I / P
   w.ue((uint32_t)sp.pps_id);             // pic_parameter_set_id
@@ -198,14 +195,29 @@ void write_slice(const StreamParams& sp, const SliceState& ss, const MbOut* cons
   if (ss.idr) w.ue((uint32_t)ss.idr_pic_id);
   if (!ss.idr) {
     w.bit(1); w.ue(0);                   // num_ref_idx_active_override_flag, num_ref_idx_l0_active_minus1
-    w.bit(1); w.ue(0); w.ue(0); w.ue(3); // ref_pic_list_modification: one (idc 0, abs_diff 1) command, end
-    w.bit(0);                            // adaptive_ref_pic_marking_mode_flag
+    w.bit(1);                            // ref_pic_list_modification_flag_l0: one command, then 3
+    w.ue((uint32_t)ss.mod_idc); w.ue((uint32_t)ss.mod_val); w.ue(3);
+    w.bit(ss.n_mmco > 0);                // adaptive_ref_pic_marking_mode_flag
+    for (int i = 0; i < ss.n_mmco; i++) {
+      const int op = ss.mmco[i][0];
+      w.ue((uint32_t)op);
+      w.ue((uint32_t)ss.mmco[i][1]);     // difference_of_pic_nums_minus1 (1, 3), long_term_frame_idx (6), max_long_term_frame_idx_plus1 (4)
+      if (op == 3) w.ue((uint32_t)ss.mmco[i][2]);   // long_term_frame_idx
+    }
+    if (ss.n_mmco > 0) w.ue(0);
+    if (sp.entropy_cabac) w.ue(0);       // cabac_init_idc (SSlice::iCabacInitIdc stays 0)
   } else {
-    w.bit(0); w.bit(0);                  // no_output_of_prior_pics_flag, long_term_reference_flag
+    w.bit(0); w.bit(ss.long_term_reference_flag);   // no_output_of_prior_pics_flag, long_term_reference_flag
   }
   w.se(ss.qp - 26);                      // slice_qp_delta
   w.ue((uint32_t)sp.dbk_idc);            // disable_deblocking_filter_idc; the offsets only with the filter on (svc_encode_slice.cpp:404-410)
   if (sp.dbk_idc != 1) { w.se(sp.dbk_alpha_div2); w.se(sp.dbk_beta_div2); }
+}
+
+void write_slice(const StreamParams& sp, const SliceState& ss, const MbOut* const* recs, std::vector<uint8_t>* rbsp,
+                 std::vector<int32_t>* mb_bits) {
+  BitWriter w(rbsp);
+  write_slice_header(w, sp, ss);
 
   // ---- slice data ----
   const int mbw = sp.mb_w, n = sp.mb_w * sp.mb_h;

@@ -69,7 +69,14 @@ struct SliceState {
   int frame_num;
   int idr_pic_id;
   int qp;
+  // reference syntax (enc_refs.h: RefDecision); the defaults are the one-reference stream's: the previous picture, no marking
+  int mod_idc = 0, mod_val = 0;         // P: ref_pic_list_modification, idc 0 (abs_diff_pic_num_minus1) or 2 (long_term_pic_num)
+  bool long_term_reference_flag = false;  // IDR
+  int n_mmco = 0;                       // P: adaptive_ref_pic_marking_mode_flag = n_mmco > 0
+  int mmco[3][3] = {};                  // operation and its values, in the order they are written
 };
+// slice header up to slice_beta_offset_div2 (svc_encode_slice.cpp:275-346); both entropy modes write it
+void write_slice_header(BitWriter& w, const StreamParams& sp, const SliceState& ss);
 // slice header + all macroblocks + trailing bits of a single-slice picture
 // coded_block_pattern me(v) mapping (Rec. H.264 Table 9-4, chroma_format_idc 1): codeNum indexed by cbp (48 entries)
 const uint8_t* cbp_me_table(bool intra);

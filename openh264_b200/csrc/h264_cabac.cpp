@@ -172,23 +172,7 @@ void mvd_comp(CabacEncoder& e, int v, int ctx_base, int sum) {
 
 void write_slice_cabac(const StreamParams& sp, const SliceState& ss, const MbOut* const* recs, std::vector<uint8_t>* rbsp) {
   BitWriter w(rbsp);
-  // ---- slice header (svc_encode_slice.cpp:275-346) ----
-  w.ue(0);                               // first_mb_in_slice
-  w.ue(ss.idr ? 2 : 0);                  // slice_type: I / P
-  w.ue((uint32_t)sp.pps_id);
-  w.put(15, (uint32_t)ss.frame_num);
-  if (ss.idr) w.ue((uint32_t)ss.idr_pic_id);
-  if (!ss.idr) {
-    w.bit(1); w.ue(0);                   // num_ref_idx_active_override_flag, num_ref_idx_l0_active_minus1
-    w.bit(1); w.ue(0); w.ue(0); w.ue(3); // ref_pic_list_modification: one (idc 0, abs_diff 1) command, end
-    w.bit(0);                            // adaptive_ref_pic_marking_mode_flag
-    w.ue(0);                             // cabac_init_idc (SSlice::iCabacInitIdc stays 0)
-  } else {
-    w.bit(0); w.bit(0);                  // no_output_of_prior_pics_flag, long_term_reference_flag
-  }
-  w.se(ss.qp - 26);                      // slice_qp_delta
-  w.ue((uint32_t)sp.dbk_idc);            // disable_deblocking_filter_idc; the offsets only with the filter on (svc_encode_slice.cpp:404-410)
-  if (sp.dbk_idc != 1) { w.se(sp.dbk_alpha_div2); w.se(sp.dbk_beta_div2); }
+  write_slice_header(w, sp, ss);
   while (w.bit_pos() & 7) w.bit(1);      // cabac_alignment_one_bit
 
   CabacEncoder e(rbsp);                  // the header is byte aligned: the arithmetic coder appends whole bytes

@@ -22,6 +22,11 @@ EncPool::EncPool(const PoolKey& key, int capacity, int device) : Batcher(capacit
   cfg.intra_period = key.intra_period;
   cfg.loop_filter_idc = key.dbk_idc; cfg.loop_filter_alpha_c0_offset = key.dbk_alpha; cfg.loop_filter_beta_offset = key.dbk_beta;
   if (b2h264_enc_create(&cfg, &enc_) != 0) { enc_ = nullptr; return; }
+  if (b2h264_enc_set_references(enc_, key.num_ref_frames, key.ltr, 30) != 0) {
+    b2h264_enc_destroy(enc_);
+    enc_ = nullptr;
+    return;
+  }
   if (cudaSetDevice(device) != cudaSuccess ||
       cudaHostAlloc((void**)&pinned_, frame_bytes_ * capacity, cudaHostAllocPortable) != cudaSuccess) {
     b2h264_enc_destroy(enc_);
@@ -55,6 +60,18 @@ int EncPool::upload(int slot) {
 
 int EncPool::force_idr(int slot) {
   return when_idle([&] { return b2h264_enc_force_idr(enc_, slot); });
+}
+
+int EncPool::ltr_recovery_request(int slot, int type, int idr_pic_id, int cur_frame_num, int last_correct_frame_num) {
+  return when_idle([&] { return b2h264_enc_ltr_recovery_request(enc_, slot, type, idr_pic_id, cur_frame_num, last_correct_frame_num); });
+}
+
+int EncPool::ltr_marking_feedback(int slot, int type, int idr_pic_id, int ltr_frame_num) {
+  return when_idle([&] { return b2h264_enc_ltr_marking_feedback(enc_, slot, type, idr_pic_id, ltr_frame_num); });
+}
+
+int EncPool::ltr_mark_period(int slot, int period) {
+  return when_idle([&] { return b2h264_enc_ltr_mark_period(enc_, slot, period); });
 }
 
 void EncPool::code_batch(const std::vector<int>& slots, int* result) {

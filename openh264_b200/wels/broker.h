@@ -29,11 +29,14 @@ namespace b2wels {
 
 struct PoolKey {
   int width, height, qp, bitrate, strategy, complexity_low, entropy_cabac, profile_idc, intra_period, dbk_idc, dbk_alpha, dbk_beta;
+  // resolved reference configuration (max_num_ref_frames of the SPS, LTR on / off): every stream of a pool has the same picture
+  // store; the LTR marking period is per stream (EncPool::ltr_mark_period)
+  int num_ref_frames = 1, ltr = 0;
   float fps;
   bool operator==(const PoolKey& o) const {
     return width == o.width && height == o.height && qp == o.qp && bitrate == o.bitrate && strategy == o.strategy && complexity_low == o.complexity_low && entropy_cabac == o.entropy_cabac &&
            profile_idc == o.profile_idc && intra_period == o.intra_period && dbk_idc == o.dbk_idc &&
-           dbk_alpha == o.dbk_alpha && dbk_beta == o.dbk_beta && fps == o.fps;
+           dbk_alpha == o.dbk_alpha && dbk_beta == o.dbk_beta && num_ref_frames == o.num_ref_frames && ltr == o.ltr && fps == o.fps;
   }
 };
 
@@ -52,6 +55,12 @@ class EncPool : public Batcher {
   // 0 or a negative / CUDA error
   int encode(int slot, std::vector<uint8_t>* au, bool* idr);
   int force_idr(int slot);
+  // loss-recovery feedback and the marking period of the slot's stream: they take effect on its next picture
+  int ltr_recovery_request(int slot, int type, int idr_pic_id, int cur_frame_num, int last_correct_frame_num);
+  int ltr_marking_feedback(int slot, int type, int idr_pic_id, int ltr_frame_num);
+  int ltr_mark_period(int slot, int period);
+  // the resolved reference configuration (b2h264_enc_get_references)
+  int references(int32_t* out4) { return b2h264_enc_get_references(enc_, out4); }
 
  private:
   void code_batch(const std::vector<int>& slots, int* result) override;

@@ -12,6 +12,7 @@
 
 #include <vector>
 
+#include "../csrc/enc_refs.h"
 #include "b2h264_codec.h"
 #include "broker.h"
 #include "codec_api.h"
@@ -20,6 +21,7 @@
 namespace {
 
 const int kMaxFps = 60, kMinFps = 1;          // MAX_FRAME_RATE / MIN_FRAME_RATE (codec/encoder/core/inc/wels_const.h:60-61)
+const int kMaxRefCamera = 10;                 // MAX_REFERENCE_PICTURE_COUNT_NUM_CAMERA (wels_const.h:127)
 
 void why(const char* msg) { fprintf(stderr, "[b2h264] unsupported encoder configuration: %s\n", msg); }
 
@@ -64,7 +66,8 @@ class B2Encoder : public ISVCEncoder {
     REQUIRE(p->iSpatialLayerNum == 1 && p->iTemporalLayerNum == 1, "more than one spatial/temporal layer");
     REQUIRE(p->iRCMode == RC_OFF_MODE, "iRCMode != RC_OFF_MODE");
     REQUIRE(l.sSliceArgument.uiSliceMode == SM_SINGLE_SLICE, "uiSliceMode != SM_SINGLE_SLICE");
-    REQUIRE(p->iNumRefFrame == 1 || p->iNumRefFrame == AUTO_REF_PIC_COUNT, "iNumRefFrame != 1");
+    REQUIRE(p->iNumRefFrame == AUTO_REF_PIC_COUNT || (p->iNumRefFrame >= 1 && p->iNumRefFrame <= kMaxRefCamera),
+            "iNumRefFrame outside 1..10 and not AUTO_REF_PIC_COUNT");
     if (p->iLoopFilterDisableIdc < 0 || p->iLoopFilterDisableIdc > 2 || p->iLoopFilterAlphaC0Offset < -6 || p->iLoopFilterAlphaC0Offset > 6 ||
         p->iLoopFilterBetaOffset < -6 || p->iLoopFilterBetaOffset > 6) return cmInitParaError;       // encoder_ext.cpp:316-323
     REQUIRE(p->iComplexityMode == LOW_COMPLEXITY || p->iComplexityMode == MEDIUM_COMPLEXITY || p->iComplexityMode == HIGH_COMPLEXITY,
@@ -74,7 +77,7 @@ class B2Encoder : public ISVCEncoder {
     // resolved parameters report it off.  iMinQp / iMaxQp only bound rate control, which is off here.
     REQUIRE(!p->bEnableDenoise && !p->bEnableBackgroundDetection && !p->bEnableSceneChangeDetect,
             "denoise / background detection / scene change detection enabled");
-    REQUIRE(!p->bEnableLongTermReference && !p->bEnableFrameSkip, "LTR or frame skip enabled");
+    REQUIRE(!p->bEnableFrameSkip, "frame skip enabled");
     REQUIRE(p->bEnableFrameCroppingFlag, "bEnableFrameCroppingFlag false");
     REQUIRE(!p->bEnableSSEI && !p->bSimulcastAVC && !p->bPrefixNalAddingCtrl, "SSEI / simulcast / prefix NAL");
     REQUIRE(p->eSpsPpsIdStrategy == CONSTANT_ID || p->eSpsPpsIdStrategy == INCREASING_ID, "eSpsPpsIdStrategy");
@@ -107,13 +110,30 @@ class B2Encoder : public ISVCEncoder {
     key.profile_idc = (int)l.uiProfileIdc;
     key.dbk_idc = p->iLoopFilterDisableIdc; key.dbk_alpha = p->iLoopFilterAlphaC0Offset; key.dbk_beta = p->iLoopFilterBetaOffset;
     key.intra_period = p->uiIntraPeriod == (unsigned int)-1 ? 0 : (int)p->uiIntraPeriod;       // param_svc.h:370-372 (GOP size 1: no rounding)
+    // reference pictures, resolved as the reference resolves them (au_set.cpp:88-133; camera LTR always keeps LONG_TERM_REF_NUM = 2
+    // long-term pictures whatever iLTRRefNum asks): the pool is keyed on what reaches the bitstream and the picture store.  The
+    // marking period is the stream's own (set below)
+    b2h264::RefConfig rc;
+    if (!b2h264::RefConfig::resolve(p->iNumRefFrame, p->bEnableLongTermReference, p->iLtrMarkPeriod, key.intra_period, &rc))
+      return cmInitParaError;
+    const int period = rc.ltr_mark_period;
+    key.num_ref_frames = rc.sps_num_ref_frames;
+    key.ltr = rc.ltr ? 1 : 0;
     pool_ = b2wels::Broker::get().attach(key, &slot_);
     if (!pool_ || slot_ < 0) { pool_.reset(); slot_ = -1; return cmMallocMemeError; }
+    if (pool_->ltr_mark_period(slot_, period) != 0) { Uninitialize(); return cmInitParaError; }
     par_ = *p;
+    par_.iLtrMarkPeriod = period;
     // what GetOption(ENCODER_OPTION_SVC_ENCODE_PARAM_EXT) reports is the RESOLVED configuration, as with the reference
     // (param_svc.h:370-372, encoder_ext.cpp:126-141,652-664)
     if (par_.uiIntraPeriod == (unsigned int)-1) par_.uiIntraPeriod = 0;
     par_.bEnableAdaptiveQuant = false;
+    {
+      int32_t r[4];
+      pool_->references(r);
+      par_.iNumRefFrame = r[0];
+      par_.iLTRRefNum = r[2];
+    }
     {
       EProfileIdc& pr = par_.sSpatialLayers[0].uiProfileIdc;
       if (pr != PRO_BASELINE && pr != PRO_MAIN && pr != PRO_HIGH) pr = PRO_UNKNOWN;
@@ -182,6 +202,36 @@ class B2Encoder : public ISVCEncoder {
         const int want = *(int*)v == -1 ? 0 : *(int*)v;
         if (want == (int)par_.uiIntraPeriod) return cmResultSuccess;
         why("ENCODER_OPTION_IDR_INTERVAL: changing uiIntraPeriod of a running stream (set it in InitializeExt)");
+        return cmUnsupportedData;
+      }
+      case ENCODER_LTR_RECOVERY_REQUEST: {
+        if (!pool_) return cmInitExpected;
+        const SLTRRecoverRequest* r = (const SLTRRecoverRequest*)v;
+        // with LTR off any request asks for an IDR; with it on, a request for another layer is dropped (ref_list_mgr_svc.cpp:519-528)
+        if (par_.bEnableLongTermReference && r->iLayerId != 0) return cmResultSuccess;
+        return pool_->ltr_recovery_request(slot_, (int)r->uiFeedbackType, (int)r->uiIDRPicId, r->iCurrentFrameNum, r->iLastCorrectFrameNum) == 0
+                   ? cmResultSuccess : cmUnknownReason;
+      }
+      case ENCODER_LTR_MARKING_FEEDBACK: {
+        if (!pool_) return cmInitExpected;
+        const SLTRMarkingFeedback* f = (const SLTRMarkingFeedback*)v;
+        if (f->iLayerId != 0) return cmResultSuccess;
+        return pool_->ltr_marking_feedback(slot_, (int)f->uiFeedbackType, (int)f->uiIDRPicId, f->iLTRFrameNum) == 0 ? cmResultSuccess : cmUnknownReason;
+      }
+      case ENCODER_LTR_MARKING_PERIOD: {
+        if (!pool_) return cmInitExpected;
+        const int period = (int)*(uint32_t*)v;
+        if (pool_->ltr_mark_period(slot_, period) != 0) return cmInitParaError;
+        par_.iLtrMarkPeriod = period;
+        return cmResultSuccess;
+      }
+      case ENCODER_OPTION_LTR: {
+        // switching LTR on or off rebuilds the reference's encoder (WelsEncoderApplyLTR -> WelsEncoderParamAdjust); here it would move
+        // the stream to another pool.  Asking for what the stream already has is accepted (camera: iLTRRefNum is always 2).
+        if (!pool_) return cmInitExpected;
+        const SLTRConfig* c = (const SLTRConfig*)v;
+        if (c->bEnableLongTermReference == par_.bEnableLongTermReference) return cmResultSuccess;
+        why("ENCODER_OPTION_LTR: switching LTR on a running stream (set bEnableLongTermReference in InitializeExt)");
         return cmUnsupportedData;
       }
       default:

@@ -112,7 +112,7 @@ def dump(bs, verbose=True):
                         while True:
                             op = r.ue()
                             if op == 0: break
-                            ops.append((op, r.ue()))
+                            ops.append((op, r.ue(), r.ue()) if op == 3 else (op, r.ue()))
                         info["mmco"] = ops
             info["qp_delta"] = r.se()
             info["dbf_idc"] = r.ue()
