@@ -120,6 +120,25 @@ int b2h264_k_downsample (int mode, uint8_t* dst, int dst_stride, int dst_w, int 
 /* the function CDownsampling::Process (downsample.cpp:143-215) picks for a plane: 0..2 dyadic forms, else 3 (luma) / 4 (chroma) */
 int b2h264_downsample_mode (int src_w, int src_h, int dst_w, int dst_h, int is_chroma);
 
+/* One destination plane of a down-sampling ladder.  mode: b2h264_downsample_mode; sx / sy: the general ratio's fixed-point steps
+ * (modes 3 and 4: WELS_ROUND(src / dst * 2^16) horizontally for luma, 2^15 otherwise; 0 for modes 0-2); src_offset /
+ * dst_offset: the plane's first byte inside one picture; row0: the plane's first row in the launch (0 for the first descriptor,
+ * then the previous descriptor's row0 + dst_h). */
+typedef struct {
+  int32_t  mode, sx, sy;
+  int32_t  src_w, src_h, src_stride;
+  int32_t  dst_w, dst_h, dst_stride;
+  int32_t  row0;
+  uint64_t src_offset, dst_offset;
+} b2h264_ds_plane;
+#define B2H264_LADDER_MAX_PLANES 24      /* 8 rungs x 3 planes */
+
+/* Every plane of every rung for the pictures of streams [lo, lo + cnt) in one launch: picture s is read at src + s * src_pitch
+ * and written at dst + s * dst_pitch, plane k at its offsets.  h_planes is a HOST array of n_planes (1..24) descriptors;
+ * descriptors with an invalid mode, an empty size or a row0 that is not the running sum of dst_h are refused (cudaErrorInvalidValue). */
+int b2h264_k_downsample_ladder (const b2h264_ds_plane* h_planes, int n_planes, uint8_t* dst, size_t dst_pitch, const uint8_t* src,
+                                size_t src_pitch, int lo, int cnt, void* stream);
+
 /* ---- WelsMotionEstimateSearch (svc_motion_estimate.cpp:170) --------------------------------- */
 typedef struct {
   int32_t blk;

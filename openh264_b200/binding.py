@@ -36,6 +36,13 @@ class MeResult(C.Structure):
                 ("ref_off", C.c_int32)]
 
 
+class DsPlane(C.Structure):
+    """b2h264_ds_plane: one destination plane of b2h264_k_downsample_ladder"""
+    _fields_ = [("mode", C.c_int32), ("sx", C.c_int32), ("sy", C.c_int32), ("src_w", C.c_int32), ("src_h", C.c_int32),
+                ("src_stride", C.c_int32), ("dst_w", C.c_int32), ("dst_h", C.c_int32), ("dst_stride", C.c_int32), ("row0", C.c_int32),
+                ("src_offset", C.c_uint64), ("dst_offset", C.c_uint64)]
+
+
 # every symbol include/b2h264.h declares: name -> argtypes (restype int unless noted)
 API = {
     "b2h264_init": [C.c_int],
@@ -70,6 +77,7 @@ API = {
     "b2h264_k_expand_plane": [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp],
     "b2h264_k_downsample": [C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_size_t, vp],
     "b2h264_downsample_mode": [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int],
+    "b2h264_k_downsample_ladder": [vp, C.c_int, vp, C.c_size_t, vp, C.c_size_t, C.c_int, C.c_int, vp],
     "b2h264_k_me_search": [vp, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp],
     "b2h264_k_me_cross_search": [vp, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp],
     "b2h264_k_weighted_pred": [C.c_int, vp, vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp],
