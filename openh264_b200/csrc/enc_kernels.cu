@@ -19,7 +19,9 @@
 #include "enc_deblock.cuh"
 #include "enc_frame.cuh"
 #include "dec_mb.cuh"
+#include "dec_records_check.h"
 #include "enc_launch.h"
+#include "enc_host.h"
 
 using namespace mbk;
 
@@ -1175,6 +1177,96 @@ __global__ void __launch_bounds__(256) k_unpack_records(const uint4* __restrict_
 int dec_launch_unpack(const void* d_pack, size_t stream_stride_bytes, const int32_t* d_idx, MbOut* d_recs, int n_streams, int n_mb, cudaStream_t st) {
   k_unpack_records<<<dim3((n_mb + 7) / 8, n_streams), 256, 0, st>>>(reinterpret_cast<const uint4*>(d_pack), stream_stride_bytes / 16, d_idx, d_recs, n_mb);
   return b2h264_launched();
+}
+
+// Test hook (not part of the public headers): the decoder's construct stage on given records, with the production hand-over and
+// launches: pack_records_compact -> dec_launch_unpack, border replication of the reference pictures, dec_launch_frame without
+// deblocking.  n streams of mb_w x mb_h macroblocks; host arrays, stream-major: recs / aux = n * mb_w * mb_h records, aux_b = as
+// many list-1 records or NULL (required when a record is B), cqp_off[s] = chroma_qp_index_offset of stream s, refs = n * n_refs
+// dense I420 pictures (16 mb_w x 16 mb_h luma) that become picture slots 0 .. n_refs - 1; the picture is decoded into slot n_refs.
+// Out (host): planes = n padded pictures (Y: (16 mb_w + 64) x (16 mb_h + 64), sample (0, 0) at row 32, column 32; Cb, Cr:
+// (8 mb_w + 32) x (8 mb_h + 32) at 16, 16), mbi = the n * mb_w * mb_h MbInfo records.  Returns -1 without launching for a bad
+// argument (dec_records_check.h), else the CUDA status.
+extern "C" int b2h264_debug_decode_records(int n, int mb_w, int mb_h, const int* cqp_off, const MbOut* recs, const DecMbAux* aux,
+                                           const DecMbAuxB* aux_b, int n_refs, const uint8_t* refs, uint8_t* planes, MbInfo* mbi) {
+  if (!dec_records_ok(n, mb_w, mb_h, cqp_off, recs, aux, aux_b, n_refs, refs, planes, mbi)) return -1;
+  const int n_mb = mb_w * mb_h;
+  bool has_b = false;
+  for (size_t i = 0; i < (size_t)n * n_mb; i++) has_b = has_b || MBT_IS_B(recs[i].mb_type);
+  const int sty = mb_w * 16 + 64, stc = mb_w * 8 + 32;
+  const size_t y_bytes = (size_t)sty * (mb_h * 16 + 64), c_bytes = (size_t)stc * (mb_h * 8 + 32), pic_bytes = y_bytes + 2 * c_bytes;
+  const size_t slots = (size_t)n_refs + 1, dense = (size_t)n_mb * 384;
+  uint8_t *d_pic = nullptr, *d_pack = nullptr;
+  int32_t* d_idx = nullptr;
+  int* d_ws = nullptr;
+  MbOut* d_recs = nullptr;
+  DecMbAux* d_aux = nullptr;
+  DecMbAuxB* d_aux_b = nullptr;
+  MbInfo* d_mbi = nullptr;
+  StreamFrame* d_sf = nullptr;
+  std::vector<uint8_t> pack((size_t)n * n_mb * sizeof(MbOut));
+  std::vector<int32_t> idx((size_t)n * n_mb);
+  std::vector<StreamFrame> h((size_t)n * n_refs);
+  auto plane0 = [&](uint8_t* base, size_t s, size_t slot, int pl) {
+    uint8_t* p = base + (s * slots + slot) * pic_bytes;
+    return pl == 0 ? p + (size_t)32 * sty + 32 : p + y_bytes + (size_t)(pl - 1) * c_bytes + (size_t)16 * stc + 16;
+  };
+  int rc = (int)cudaMalloc(&d_pic, (size_t)n * slots * pic_bytes + 256);
+  if (!rc) rc = (int)cudaMemset(d_pic, 0, (size_t)n * slots * pic_bytes + 256);
+  if (!rc) rc = (int)cudaMalloc(&d_pack, pack.size());
+  if (!rc) rc = (int)cudaMalloc(&d_idx, idx.size() * sizeof(int32_t));
+  if (!rc) rc = (int)cudaMalloc(&d_recs, (size_t)n * n_mb * sizeof(MbOut));
+  if (!rc) rc = (int)cudaMalloc(&d_aux, (size_t)n * n_mb * sizeof(DecMbAux));
+  if (!rc && has_b) rc = (int)cudaMalloc(&d_aux_b, (size_t)n * n_mb * sizeof(DecMbAuxB));
+  if (!rc) rc = (int)cudaMalloc(&d_mbi, (size_t)n * n_mb * sizeof(MbInfo));
+  if (!rc) rc = (int)cudaMemset(d_mbi, 0, (size_t)n * n_mb * sizeof(MbInfo));
+  if (!rc) rc = (int)cudaMalloc(&d_sf, h.size() * sizeof(StreamFrame));
+  if (!rc) rc = (int)cudaMalloc(&d_ws, dec_sched_ints(n, mb_w, mb_h) * sizeof(int));
+  // the reference pictures into their slots, then their borders as the decoder replicates them after decoding a picture
+  for (size_t s = 0; s < (size_t)n && !rc; s++)
+    for (size_t r = 0; r < (size_t)n_refs && !rc; r++) {
+      const uint8_t* src = refs + (s * n_refs + r) * dense;
+      for (int pl = 0; pl < 3 && !rc; pl++) {
+        const int w = pl ? 8 * mb_w : 16 * mb_w, hh = pl ? 8 * mb_h : 16 * mb_h;
+        rc = (int)cudaMemcpy2D(plane0(d_pic, s, r, pl), pl ? stc : sty, src + (pl ? (size_t)n_mb * 256 + (size_t)(pl - 1) * n_mb * 64 : 0), w, w, hh,
+                               cudaMemcpyHostToDevice);
+      }
+      StreamFrame& F = h[s * n_refs + r];
+      memset(&F, 0, sizeof(F));
+      F.p.mb_w = mb_w; F.p.mb_h = mb_h; F.p.rec_stride_y = sty; F.p.rec_stride_c = stc;
+      for (int pl = 0; pl < 3; pl++) F.f.rec[pl] = plane0(d_pic, s, r, pl);
+    }
+  if (!rc) rc = (int)cudaMemcpy(d_sf, h.data(), h.size() * sizeof(StreamFrame), cudaMemcpyHostToDevice);
+  if (!rc) rc = launch_expand(d_sf, n * n_refs, mb_w, mb_h, 0);
+  if (!rc) rc = (int)cudaDeviceSynchronize();
+  // the records: compact form per stream, unpacked on the device as b2h264_dec_decode does it
+  for (int s = 0; s < n && !rc; s++) {
+    const int units = b2h264::pack_records_compact(recs + (size_t)s * n_mb, n_mb, pack.data() + (size_t)s * n_mb * sizeof(MbOut), idx.data() + (size_t)s * n_mb);
+    if (units > 0)
+      rc = (int)cudaMemcpy(d_pack + (size_t)s * n_mb * sizeof(MbOut), pack.data() + (size_t)s * n_mb * sizeof(MbOut), (size_t)units * 32, cudaMemcpyHostToDevice);
+  }
+  if (!rc) rc = (int)cudaMemcpy(d_idx, idx.data(), idx.size() * sizeof(int32_t), cudaMemcpyHostToDevice);
+  if (!rc) rc = dec_launch_unpack(d_pack, (size_t)n_mb * sizeof(MbOut), d_idx, d_recs, n, n_mb, 0);
+  if (!rc) rc = (int)cudaMemcpy(d_aux, aux, (size_t)n * n_mb * sizeof(DecMbAux), cudaMemcpyHostToDevice);
+  if (!rc && has_b) rc = (int)cudaMemcpy(d_aux_b, aux_b, (size_t)n * n_mb * sizeof(DecMbAuxB), cudaMemcpyHostToDevice);
+  for (int s = 0; s < n && !rc; s++) {
+    StreamFrame& F = h[s];
+    memset(&F, 0, sizeof(F));
+    F.p.mb_w = mb_w; F.p.mb_h = mb_h; F.p.rec_stride_y = sty; F.p.rec_stride_c = stc;
+    F.p.mv_range = 64; F.p.dec_mode = 1; F.p.dec_cqp_off = cqp_off[s];
+    for (int pl = 0; pl < 3; pl++) { F.f.rec[pl] = plane0(d_pic, s, n_refs, pl); F.f.ref[pl] = F.f.dpb0[pl] = plane0(d_pic, s, 0, pl); }
+    F.f.dpb_stride = (int64_t)pic_bytes;
+    F.f.mbi = d_mbi + (size_t)s * n_mb;
+    F.f.dec_aux_b = has_b ? d_aux_b + (size_t)s * n_mb : nullptr;
+  }
+  if (!rc) rc = (int)cudaMemcpy(d_sf, h.data(), (size_t)n * sizeof(StreamFrame), cudaMemcpyHostToDevice);
+  if (!rc) rc = dec_launch_frame(d_sf, n, mb_w, mb_h, d_ws, d_recs, d_aux, 0, 0, has_b ? 1 : 0);
+  if (!rc) rc = (int)cudaDeviceSynchronize();
+  for (int s = 0; s < n && !rc; s++)
+    rc = (int)cudaMemcpy(planes + (size_t)s * pic_bytes, d_pic + ((size_t)s * slots + n_refs) * pic_bytes, pic_bytes, cudaMemcpyDeviceToHost);
+  if (!rc) rc = (int)cudaMemcpy(mbi, d_mbi, (size_t)n * n_mb * sizeof(MbInfo), cudaMemcpyDeviceToHost);
+  cudaFree(d_pic); cudaFree(d_pack); cudaFree(d_idx); cudaFree(d_recs); cudaFree(d_aux); cudaFree(d_aux_b); cudaFree(d_mbi); cudaFree(d_sf); cudaFree(d_ws);
+  return rc;
 }
 
 extern "C" int b2h264_debug_enc_stats(unsigned long long* out16, int reset) {

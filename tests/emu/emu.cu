@@ -198,6 +198,9 @@ void deblock_frame_host(const EncFrameParams& p, const EncFramePtrs& f) {
 
 }  // namespace
 
+// the border replication of expand_frame_host, for the hooks built beside this file (decode_records_hooks.cu)
+void emu_expand_frame(const EncFrameParams& p, const EncFramePtrs& f) { expand_frame_host(p, f); }
+
 // do two records describe the same coded macroblock?  (only what the bitstream carries is compared)
 static bool same_record(const MbOut& a, const MbOut& b) {
   bool same = a.mb_type == b.mb_type;
@@ -440,7 +443,8 @@ extern "C" int emu_deblock_picture(uint8_t* y, uint8_t* cb, uint8_t* cr, int str
 
 // ---- randomized writer <-> parser round trip (levels up to the Baseline escape range, every macroblock type) -----------
 // Returns 0, a negative ParseError, or 1 + index of the first macroblock that came back different.
-static int random_pictures(unsigned seed, int pictures, bool decodable, uint8_t* stream_out, long cap, long* stream_len);
+static int random_pictures(unsigned seed, int pictures, bool decodable, uint8_t* stream_out, long cap, long* stream_len,
+                           bool loop_filter_off = false, std::vector<b2h264::ParsedPicture>* parsed = nullptr);
 extern "C" int emu_roundtrip_random(unsigned seed, int pictures) { return random_pictures(seed, pictures, false, nullptr, 0, nullptr); }
 // the same generator restricted to streams every conforming decoder reconstructs identically (DC intra prediction only,
 // bounded coefficient energy, bounded vectors): the Annex-B stream is returned for tests/test_decoder_emu.py, which
@@ -450,12 +454,31 @@ extern "C" long emu_random_stream(unsigned seed, int pictures, uint8_t* out, lon
   const int rc = random_pictures(seed, pictures, true, out, cap, &len);
   return rc == 0 ? len : (long)rc;
 }
-static int random_pictures(unsigned seed, int pictures, bool decodable, uint8_t* stream_out, long cap, long* stream_len) {
+// the same decodable streams written with the loop filter off (disable_deblocking_filter_idc 1), and what the parser made of each
+// picture: recs / aux = pictures * 20 records (5 x 4 macroblocks, raster), info[3 * p] = the picture's slot, the stream's slot
+// count and its chroma_qp_index_offset.  tests/test_decode_records_emu.py reconstructs these pictures with the spec oracle and
+// compares them with the reference decoder's.  Returns the stream's length or a negative error as emu_random_stream does.
+extern "C" long emu_random_stream_records(unsigned seed, int pictures, uint8_t* out, long cap, MbOut* recs, DecMbAux* aux, int32_t* info) {
+  long len = 0;
+  std::vector<b2h264::ParsedPicture> parsed;
+  const int rc = random_pictures(seed, pictures, true, out, cap, &len, true, &parsed);
+  if (rc != 0) return (long)rc;
+  for (size_t p = 0; p < parsed.size(); p++) {
+    if (parsed[p].mbs.size() != 20 || parsed[p].aux.size() != 20) return -300;
+    memcpy(recs + 20 * p, parsed[p].mbs.data(), 20 * sizeof(MbOut));
+    memcpy(aux + 20 * p, parsed[p].aux.data(), 20 * sizeof(DecMbAux));
+    info[3 * p] = parsed[p].cur_slot; info[3 * p + 1] = parsed[p].n_slots; info[3 * p + 2] = parsed[p].chroma_qp_offset;
+  }
+  return len;
+}
+static int random_pictures(unsigned seed, int pictures, bool decodable, uint8_t* stream_out, long cap, long* stream_len,
+                           bool loop_filter_off, std::vector<b2h264::ParsedPicture>* parsed) {
   uint32_t x = seed * 2654435761u + 12345u;
   auto rnd = [&](uint32_t n) { x = x * 1664525u + 1013904223u; return (x >> 8) % n; };
   const int W = 5, H = 4;
   b2h264::StreamCtl ctl;
   ctl.init(W * 16, H * 16, 26, 30.0f, 0);
+  if (loop_filter_off && !ctl.set_loop_filter(1, 0, 0)) return -400;
   b2h264::ParserState st;
   int cur_qp = 26;                                            // qp the block being filled will be dequantised with
   auto rand_level = [&]() {
@@ -481,6 +504,22 @@ static int random_pictures(unsigned seed, int pictures, bool decodable, uint8_t*
         v = (int16_t)(v < 0 ? -a : a);
       }
       lv[i] = v; nz++;
+    }
+    if (loop_filter_off) {
+      // the streams written with the loop filter off must also meet 8.5.10 to 8.5.12 exactly: every value of the inverse
+      // transforms is bounded by the sum of the scaled coefficients' magnitudes, and a scaled level is at most |level| x 29 x
+      // 2^(qp / 6) (normAdjust4x4 <= 29); a block's levels keep that sum under 16000 (room for a luma / chroma DC of a
+      // quarter of it), so the spec oracle reconstructs them as the standard defines
+      const int budget = 16000 / (29 << (cur_qp / 6));
+      int sum = 0;
+      for (int i = 0; i < max_coef; i++) sum += lv[i] < 0 ? -lv[i] : lv[i];
+      while (sum > budget) {
+        int k = 0;
+        for (int i = 1; i < max_coef; i++) if (abs(lv[i]) > abs(lv[k])) k = i;
+        lv[k] = (int16_t)(lv[k] < 0 ? lv[k] + 1 : lv[k] - 1);
+        if (lv[k] == 0) nz--;
+        sum--;
+      }
     }
     return nz;
   };
@@ -571,6 +610,7 @@ static int random_pictures(unsigned seed, int pictures, bool decodable, uint8_t*
     if (got.mbs.size() != recs.size()) return -100;
     for (size_t i = 0; i < recs.size(); i++)
       if (!same_record(recs[i], got.mbs[i])) return 1 + (int)i;
+    if (parsed) parsed->push_back(got);
     if (stream_out) {
       if (*stream_len + (long)au.size() > cap) return -200;
       memcpy(stream_out + *stream_len, au.data(), au.size());
