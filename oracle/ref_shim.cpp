@@ -8,6 +8,7 @@
  * initialised with uiCpuFlag = 0 (the *_c path), so tests can diff oracle vs reference call by
  * call.  Nothing here re-implements any arithmetic.
  */
+#include <limits.h>
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
@@ -28,6 +29,10 @@
 #include "encoder_context.h"
 #include "mv_pred.h"
 #include "svc_base_layer_md.h"
+#include "get_intra_predictor.h"
+#include "svc_encode_mb.h"
+#include "svc_encode_slice.h"
+#include "encoder.h"
 
 #include "../oracle/h264_oracle.h"
 
@@ -343,6 +348,176 @@ void ref_me_cross_search (const uint8_t* cur, int cs, const uint8_t* ref, int rs
 }
 
 } // extern "C"
+
+/* The intra path of one macroblock as WelsMdIntraMb (svc_base_layer_md.cpp:956) runs it for stage I, and as
+ * WelsMdFirstIntraMode (:1829) runs it for stage C once I16x16 has beaten the inter cost: WelsMdI16x16, then
+ * WelsMdIntraSecondaryModesEnc (:2023) = pfIntraFineMd (WelsMdI4x4, or the texture gate MdIntraAnalysisVaaInfo plus
+ * WelsMdI4x4Fast in LOW complexity), WelsEncRecI16x16Y when I16x16 stays, WelsMdIntraChroma and WelsIMbChromaEncode.
+ * Driven with a minimal encoder context in the style of ref_pskip and the C function table (the C-only build leaves
+ * pfIntra16x16Combined3 / pfIntra8x8Combined3 / pfIntra4x4Combined3 unset, so the mode loops run).
+ *
+ * in / out: the case and result records of b2h264_debug_intra_tail (openh264_b200/csrc/enc_kernels.cu), n of each.  The
+ * macroblock sits at (1, 1) of a 3 x 2 macroblock reconstructed picture; the case's neighbour samples go where their
+ * neighbour is available and every other sample of that picture, including the macroblock itself, gets pseudo-random bytes, so
+ * a predictor that reads a neighbour it must not use changes the result.  The neighbours' I4x4 modes reach the mode cache
+ * through FillNeighborCacheIntra (md.cpp:51).  The output record holds what the reference computed in the product's layouts
+ * (MbOut: modes, prev / rem flags, levels; MbInfo: nnz, i4_mode, mb_type, cbp; the tail: cost limit used, I4x4 cost or
+ * INT_MAX when the try did not run, lambda, 0; the reconstruction tile).  Fields the reference leaves stale (rem flags of
+ * predicted modes, AC entry 15, the I16x16 DC of an I4x4 macroblock) are copied as the reference has them.
+ * costs[3 i]: I16x16 cost, I4x4 cost (INT_MAX: not tried), chroma cost.  Returns -1 for a bad argument. */
+namespace {
+enum { kTyPitch = 32, kTcPitch = 16, kTile = 17 * 32 + 2 * 9 * 16, kIn = kTile + 384 + 32, kOutMbOut = 896, kOutInfo = 120,
+       kOut = kOutMbOut + kOutInfo + 16 + kTile };
+int32_t g_cost4;
+int32_t FineMdRecordingCost (sWelsEncCtx* ctx, SWelsMD* md, SMB* mb, SMbCache* cache) {
+  /* WelsMdIntraFinePartition[Vaa] (:932, :942), keeping the I4x4 cost that they fold into iCostLuma */
+  const bool fast = ctx->pFuncList->sSampleDealingFuncs.pfMdCost == ctx->pFuncList->sSampleDealingFuncs.pfSampleSad;
+  g_cost4 = INT_MAX;
+  if (!fast) g_cost4 = WelsMdI4x4 (ctx, md, mb, cache);
+  else if (MdIntraAnalysisVaaInfo (ctx, cache->SPicData.pEncMb[0])) g_cost4 = WelsMdI4x4Fast (ctx, md, mb, cache);
+  if (g_cost4 < md->iCostLuma) {
+    mb->uiMbType = MB_TYPE_INTRA4x4;
+    md->iCostLuma = g_cost4;
+  }
+  return md->iCostLuma;
+}
+}  // namespace
+
+extern "C" int ref_intra_mb (int n, const uint8_t* in, uint8_t* out, int32_t* costs) {
+  if (n < 1 || !in || !out) return -1;
+  SWelsFuncPtrList* f = Funcs();
+  WelsInitIntraPredFuncs (f, 0);
+  InitIntraAnalysisVaaInfo (f, 0);
+  f->pfSetMemZeroSize8 = f->pfSetMemZeroSize64 = WelsSetMemZero_c;   /* InitFunctionPointers (encoder.cpp:157) */
+  f->pfIntraFineMd = FineMdRecordingCost;
+  static int32_t enc_offs[24], dec_offs[24];
+  static SStrideTables tabs;
+  static SDqLayer layer;
+  static sWelsEncCtx ctx;
+  static SDCTCoeff dct;
+  const int ys = 64, cs = 32;                                       /* reconstructed picture: 48 x 32 luma at stride 64 */
+  alignas (16) static uint8_t rec[32 * 64 + 2 * 16 * 32];
+  alignas (16) static uint8_t src[16 * 16 + 2 * 8 * 8];
+  alignas (16) static int16_t coef[384];
+  alignas (16) static uint8_t pred_mb[2 * 256], pred_blk4[2 * 16];
+  static bool prev_flag[16];
+  static int8_t rem_flag[16];
+  WelsGetEncBlockStrideOffset (enc_offs, 16, 8);
+  WelsGetEncBlockStrideOffset (dec_offs, ys, cs);
+  tabs.pStrideEncBlockOffset[0] = enc_offs;
+  tabs.pStrideDecBlockOffset[0][1] = dec_offs;                      /* [did][temporal id == 0] */
+  layer.iEncStride[0] = 16; layer.iEncStride[1] = layer.iEncStride[2] = 8;
+  layer.iCsStride[0] = ys; layer.iCsStride[1] = layer.iCsStride[2] = cs;
+  layer.iMbWidth = 2;
+  ctx.pCurDqLayer = &layer;
+  ctx.pFuncList = f;
+  ctx.pStrideTab = &tabs;
+  ctx.uiDependencyId = 0; ctx.uiTemporalId = 0;
+  uint32_t seed = 0x9e3779b9u;
+  for (int i = 0; i < n; i++) {
+    const uint8_t* c = in + (size_t) kIn * i;
+    const int32_t* prm = (const int32_t*) (c + kTile + 384);
+    const int8_t* nm = (const int8_t*) (c + kTile + 400);
+    const int qp = prm[0], nb = prm[1], fast = prm[2], limit = prm[3];
+    if (qp < 0 || qp > 51 || nb < 0 || nb > 15) return -1;
+    const uint8_t* ty = c;
+    const uint8_t* tc[2] = {c + 17 * kTyPitch, c + 17 * kTyPitch + 9 * kTcPitch};
+    for (size_t k = 0; k < sizeof (rec); k++) { seed = seed * 1664525u + 1013904223u; rec[k] = (uint8_t) (seed >> 24); }
+    uint8_t* py = rec + 16 * ys + 16;                                /* the macroblock at (1, 1) */
+    uint8_t* pc[2] = {rec + 32 * ys + 8 * cs + 8, rec + 32 * ys + 16 * cs + 8 * cs + 8};
+    if (nb & 4) py[-ys - 1] = ty[0];
+    for (int x = 0; x < 16; x++) if (nb & 2) py[-ys + x] = ty[1 + x];
+    for (int x = 16; x < 24; x++) if (nb & 8) py[-ys + x] = ty[1 + x];
+    for (int y = 0; y < 16; y++) if (nb & 1) py[y * ys - 1] = ty[(y + 1) * kTyPitch];
+    for (int p = 0; p < 2; p++) {
+      if (nb & 4) pc[p][-cs - 1] = tc[p][0];
+      for (int x = 0; x < 8; x++) if (nb & 2) pc[p][-cs + x] = tc[p][1 + x];
+      for (int y = 0; y < 8; y++) if (nb & 1) pc[p][y * cs - 1] = tc[p][(y + 1) * kTcPitch];
+    }
+    memcpy (src, c + kTile, 384);
+    /* macroblocks 0 top-left, 1 top, 2 left, 3 current of a 2-wide array (the current one's top-right neighbour is only a bit) */
+    SMB mbs[4];
+    int8_t modes[4 * INTRA_4x4_MODE_NUM], nnz[4 * MB_LUMA_CHROMA_BLOCK4x4_NUM];
+    int32_t sad[4];
+    memset (mbs, 0, sizeof (mbs));
+    memset (modes, 0, sizeof (modes));
+    memset (nnz, 0, sizeof (nnz));
+    for (int k = 0; k < 4; k++) {
+      mbs[k].pIntra4x4PredMode = modes + INTRA_4x4_MODE_NUM * k;
+      mbs[k].pNonZeroCount = nnz + MB_LUMA_CHROMA_BLOCK4x4_NUM * k;
+      mbs[k].pSadCost = sad + k;
+      mbs[k].uiMbType = MB_TYPE_INTRA16x16;
+    }
+    if (nm[0] >= 0) {                                                /* left: right column, rows 0..3 (pIntra4x4PredMode[4, 5, 6, 3]) */
+      mbs[2].uiMbType = MB_TYPE_INTRA4x4;
+      mbs[2].pIntra4x4PredMode[4] = nm[0]; mbs[2].pIntra4x4PredMode[5] = nm[1];
+      mbs[2].pIntra4x4PredMode[6] = nm[2]; mbs[2].pIntra4x4PredMode[3] = nm[3];
+    }
+    if (nm[4] >= 0) {                                                /* top: bottom row (pIntra4x4PredMode[0..3]) */
+      mbs[1].uiMbType = MB_TYPE_INTRA4x4;
+      for (int x = 0; x < 4; x++) mbs[1].pIntra4x4PredMode[x] = nm[4 + x];
+    }
+    SMB* mb = &mbs[3];
+    mb->iMbX = 1; mb->iMbY = 1; mb->iMbXY = 3;
+    mb->uiLumaQp = (uint8_t) qp;
+    mb->uiChromaQp = WelsCommon::g_kuiChromaQpTable[qp];
+    mb->uiNeighborAvail = (uint8_t) ((nb & 3) | ((nb & 4) ? TOPLEFT_MB_POS : 0) | ((nb & 8) ? TOPRIGHT_MB_POS : 0));
+    SMbCache cache;
+    memset (&cache, 0, sizeof (cache));
+    memset (&dct, 0, sizeof (dct));
+    memset (coef, 0, sizeof (coef));
+    memset (prev_flag, 0, sizeof (prev_flag));
+    memset (rem_flag, 0, sizeof (rem_flag));
+    cache.pCoeffLevel = coef;
+    cache.pDct = &dct;
+    cache.pMemPredMb = pred_mb;
+    cache.pMemPredBlk4 = pred_blk4;
+    cache.pPrevIntra4x4PredModeFlag = prev_flag;
+    cache.pRemIntra4x4PredModeFlag = rem_flag;
+    cache.SPicData.pEncMb[0] = src; cache.SPicData.pEncMb[1] = src + 256; cache.SPicData.pEncMb[2] = src + 320;
+    cache.SPicData.pCsMb[0] = py; cache.SPicData.pCsMb[1] = pc[0]; cache.SPicData.pCsMb[2] = pc[1];
+    /* WelsMdIntraInit (:259) */
+    mb->uiCbp = 0;
+    FillNeighborCacheIntra (&cache, mb, layer.iMbWidth);
+    cache.pMemPredLuma = cache.pMemPredMb;
+    cache.pMemPredChroma = cache.pMemPredMb + 256;
+    f->sSampleDealingFuncs.pfMdCost = fast ? f->sSampleDealingFuncs.pfSampleSad : f->sSampleDealingFuncs.pfSampleSatd;
+    SWelsMD md;
+    memset (&md, 0, sizeof (md));
+    md.iLambda = g_kiQpCostTable[qp];
+    const int32_t cost16 = WelsMdI16x16 (f, &layer, &cache, md.iLambda);
+    md.iCostLuma = limit < 0 ? cost16 : limit;
+    mb->uiMbType = MB_TYPE_INTRA16x16;
+    WelsMdIntraSecondaryModesEnc (&ctx, &md, mb, &cache);
+    /* ---- the result in the product's layouts ---- */
+    uint8_t* o = out + (size_t) kOut * i;
+    memset (o, 0, kOut);
+    const bool i4 = IS_INTRA4x4 (mb->uiMbType);
+    o[3] = (uint8_t) g_kiMapModeI16x16[cache.uiLumaI16x16Mode];
+    o[4] = (uint8_t) g_kiMapModeIntraChroma[cache.uiChmaI8x8Mode];
+    for (int k = 0; k < 16; k++) { o[8 + k] = (uint8_t) prev_flag[k]; o[24 + k] = (uint8_t) rem_flag[k]; }
+    memcpy (o + 80, dct.iLumaI16x16Dc, 32);
+    memcpy (o + 112, dct.iLumaBlock, 512);
+    memcpy (o + 624, dct.iChromaDc, 16);
+    memcpy (o + 640, dct.iChromaBlock, 256);
+    uint8_t* info = o + kOutMbOut;
+    int8_t* inz = (int8_t*) info + 64;
+    for (int k = 0; k < 16; k++) inz[k] = mb->pNonZeroCount[k];                          /* luma: raster in both */
+    for (int j = 0; j < 8; j++) inz[16 + j] = mb->pNonZeroCount[g_kuiMbCountScan4Idx[16 + j]];   /* chroma: 2 x 2 raster per plane */
+    for (int k = 0; k < 16; k++) ((int8_t*) info)[88 + k] = cache.iIntraPredMode[9 + (k & 3) + 8 * (k >> 2)];
+    info[112] = i4 ? 0 : 1;                                                               /* MBT_I4x4 / MBT_I16x16 */
+    info[113] = mb->uiCbp;
+    const int32_t tail[4] = {limit < 0 ? cost16 : limit, g_cost4, md.iLambda, 0};
+    memcpy (o + kOutMbOut + kOutInfo, tail, 16);
+    uint8_t* t = o + kOutMbOut + kOutInfo + 16;
+    memcpy (t, c, kTile);
+    for (int y = 0; y < 16; y++) memcpy (t + (y + 1) * kTyPitch + 1, py + y * ys, 16);
+    for (int p = 0; p < 2; p++)
+      for (int y = 0; y < 8; y++) memcpy (t + 17 * kTyPitch + 9 * kTcPitch * p + (y + 1) * kTcPitch + 1, pc[p] + y * cs, 8);
+    if (costs) { costs[3 * i] = cost16; costs[3 * i + 1] = g_cost4; costs[3 * i + 2] = md.iCostChroma; }
+  }
+  return 0;
+}
 
 /* ------------------------------------------------------------------------------------------------
  * Frame-level drivers through the reference's own PUBLIC API (codec_api.h): used as the end-to-end
