@@ -32,7 +32,13 @@ MBK_HD void mb_ctx(MbCtx& c, const EncFrameParams& p, const EncFramePtrs& f, int
 // Runs ONE stage of a macroblock (see enc_inter.cuh) and returns the stage to run next (MBS_DONE: the
 // reconstruction and the records are stored and published).  MBS_A / MBS_I are the entry stages of a P / an IDR
 // picture's macroblock: they start from an empty scratch; the others continue on the scratch the previous stage left.
+// Host build: after a stage A that ran the skip candidate's intra check it returns MBP_SKIPCAND_INTRA, and called with that
+// id it returns the stage that really follows (enc_inter.cuh: the paths keep their numbering).
 MBK_HD int mb_run_stage(const MbCtx& c, MbScratch& s, int stage) {
+#ifndef __CUDA_ARCH__
+  if (stage == MBP_SKIPCAND_INTRA) return g_skipcand_next;
+  g_skipcand_intra = false;
+#endif
   int next = MBS_DONE;
   if (stage == MBS_A || stage == MBS_I) {
     phase_mark(s, 31);
@@ -53,7 +59,7 @@ MBK_HD int mb_run_stage(const MbCtx& c, MbScratch& s, int stage) {
     intra_mb_finish(c, s, cost16, bb);
   }
   else if (stage == MBS_A) next = inter_stage_a(c, s);
-  else if (stage == MBS_B || stage == MBS_BSKIP) next = inter_stage_b(c, s);
+  else if (stage == MBS_B) next = inter_stage_b(c, s);
   else if (stage == MBS_C) next = inter_stage_c(c, s);
   warp_sync();
   if (next == MBS_DONE) {
@@ -69,6 +75,9 @@ MBK_HD int mb_run_stage(const MbCtx& c, MbScratch& s, int stage) {
     }
     phase_mark(s, 11);
   }
+#ifndef __CUDA_ARCH__
+  if (g_skipcand_intra) { g_skipcand_next = next; return MBP_SKIPCAND_INTRA; }
+#endif
   return next;
 }
 

@@ -905,11 +905,19 @@ MBK_HD void decided_pskip(const MbCtx& c, MbScratch& s) {
 // ---- the P-slice macroblock (WelsMdInterMb :1858 + WelsMdInterSecondaryModesEnc :1997) --------------------------------
 // The macroblock is coded in up to three STAGES; the device scheduler runs each stage of many macroblocks as a
 // lock-step batch (enc_kernels.cu) and parks the scratch between stages, the host build runs them back to back.
-//   A  skip test; a decided P_SKIP (left, top and top-right neighbours skipped too) ends here
-//   B  16x16 search (unless A found a skip candidate), intra-16x16 check, sub-partitions, refinement, residual
-//   C  the intra branch of a P macroblock (taken from B when intra 16x16 beats the inter cost)
+//   A  skip test; a skip candidate also takes the intra-16x16 check here and ends as P_SKIP or goes on to C
+//      (WelsMdInterMb decides it in one pass too: skip judgement, then WelsMdFirstIntraMode)
+//   B  16x16 search, intra-16x16 check, sub-partitions, refinement, residual
+//   C  the intra branch of a P macroblock (taken from A or B when intra 16x16 beats the inter cost)
 // Values that cross a stage boundary live in s.st (warp-uniform; written by lane 0).
-enum { MBS_DONE = 0, MBS_A = 1, MBS_I = 2, MBS_BSKIP = 3, MBS_B = 4, MBS_C = 5, MBS_COUNT = 6 };
+// Stage ids (each stage has a ready list, enc_kernels.cu: enc_list).  Id 3 is not a stage: the host build reports the intra
+// check of a skip candidate, which stage A runs, as a step of its own with that id (mb_run_stage), so that the paths it
+// records (bit id = the step ran: tests/emu, tools/sched_sim.py, tools/sim_data) keep the numbering of the time that check
+// was a stage (Bs).
+enum { MBS_DONE = 0, MBS_A = 1, MBS_I = 2, MBP_SKIPCAND_INTRA = 3, MBS_B = 4, MBS_C = 5, MBS_COUNT = 6 };
+// host build: stage A ran the skip candidate's intra check (set by inter_stage_a), and the stage that follows it
+inline bool g_skipcand_intra;
+inline int g_skipcand_next;
 
 // bookkeeping for the neighbours and the next frame
 MBK_FN void inter_tail(const MbCtx& c, MbScratch& s) {
@@ -961,19 +969,34 @@ MBK_STAGE int inter_stage_a(const MbCtx& c, MbScratch& s) {
     }
   }
   phase_mark(s, 2);
-  if (is_skip && keep_skip) {
+  if (is_skip && !keep_skip) {
+    // intra check of a skip candidate (WelsMdFirstIntraMode :1829): the skip test wrote skip_pred and the refinement planes
+    // only, so the tile borders and cur_y are still those mb_load_all staged
+#ifndef __CUDA_ARCH__
+    g_skipcand_intra = true;
+#endif
+    int bb;
+    const int cost16 = md_i16x16_inl(c, s, &bb);
+    phase_mark(s, 4);
+    if (cost16 < cost_luma) {
+      st_save(s, 1, cost_luma, cost_skip_mb, p16_mvx, p16_mvy, MBT_P16x16);
+      if (lane_id() == 0) { s.st.cost16 = cost16; s.st.bb = bb; }
+      warp_sync();
+      return MBS_C;
+    }
+  }
+  if (is_skip) {
     decided_pskip(c, s);
     st_save(s, 1, cost_luma, cost_skip_mb, p16_mvx, p16_mvy, MBT_PSKIP);
     inter_tail(c, s);
     return MBS_DONE;
   }
-  st_save(s, is_skip ? 1 : 0, cost_luma, cost_skip_mb, p16_mvx, p16_mvy, MBT_P16x16);
-  return is_skip ? MBS_BSKIP : MBS_B;
+  st_save(s, 0, cost_luma, cost_skip_mb, p16_mvx, p16_mvy, MBT_P16x16);
+  return MBS_B;
 }
 
 MBK_STAGE int inter_stage_b(const MbCtx& c, MbScratch& s) {
   const int mbw = c.p.mb_w, idx = c.mby * mbw + c.mbx;
-  const bool is_skip = s.st.is_skip != 0;
   int cost_luma = s.st.cost_luma, cost_skip_mb = s.st.cost_skip_mb, p16_mvx = s.st.p16_mvx, p16_mvy = s.st.p16_mvy;
   MeState& me16 = s.me[0];
   MeState* me16x8 = &s.me[1];
@@ -988,49 +1011,45 @@ MBK_STAGE int inter_stage_b(const MbCtx& c, MbScratch& s) {
   // t >= 0 are the sub-partition shapes of `plan` (WelsMdInterFinePartition :1238 / WelsMdInterFinePartitionVaa :1270).
   int16_t (*mvc)[2] = s.mvcand;
   int px16 = 0, py16 = 0, n16 = 1;
-  if (!is_skip) {
-    pred_mv(s, 0, 4, 0, &px16, &py16);
-    {                                      // the window copy flies while the candidate list is put together
-      int sx, sy;
-      me_start_point(c, px16, py16, &sx, &sy);
-      win_issue(c, s, sx, sy);
-    }
-    sad_pred_mb = predict_sad(s);
-    n16 += (c.nb & NB_LEFT) ? 1 : 0;                                      // [0] = sMvBase (0,0)
-    n16 += (c.nb & NB_TOP) ? 1 : 0;
-    if (c.p.ref_is_p) { n16 += c.mbx < mbw - 1 ? 1 : 0; n16 += c.mby < c.p.mb_h - 1 ? 1 : 0; }
-    if (lane_id() == 0) {
-      int k = 0;
-      mvc[k][0] = 0; mvc[k][1] = 0; k++;
-      if (c.nb & NB_LEFT) { mvc[k][0] = s.nbi[3].p16x16_mv[0]; mvc[k][1] = s.nbi[3].p16x16_mv[1]; k++; }
-      if (c.nb & NB_TOP) { mvc[k][0] = s.nbi[1].p16x16_mv[0]; mvc[k][1] = s.nbi[1].p16x16_mv[1]; k++; }
-      if (c.p.ref_is_p) {
-        if (c.mbx < mbw - 1) { mvc[k][0] = c.f.ref_info[idx + 1].mv16[0]; mvc[k][1] = c.f.ref_info[idx + 1].mv16[1]; k++; }
-        if (c.mby < c.p.mb_h - 1) { mvc[k][0] = c.f.ref_info[idx + mbw].mv16[0]; mvc[k][1] = c.f.ref_info[idx + mbw].mv16[1]; k++; }
-      }
-    }
-    warp_sync();
-    win_wait(c, s);
+  pred_mv(s, 0, 4, 0, &px16, &py16);
+  {                                        // the window copy flies while the candidate list is put together
+    int sx, sy;
+    me_start_point(c, px16, py16, &sx, &sy);
+    win_issue(c, s, sx, sy);
   }
+  sad_pred_mb = predict_sad(s);
+  n16 += (c.nb & NB_LEFT) ? 1 : 0;                                        // [0] = sMvBase (0,0)
+  n16 += (c.nb & NB_TOP) ? 1 : 0;
+  if (c.p.ref_is_p) { n16 += c.mbx < mbw - 1 ? 1 : 0; n16 += c.mby < c.p.mb_h - 1 ? 1 : 0; }
+  if (lane_id() == 0) {
+    int k = 0;
+    mvc[k][0] = 0; mvc[k][1] = 0; k++;
+    if (c.nb & NB_LEFT) { mvc[k][0] = s.nbi[3].p16x16_mv[0]; mvc[k][1] = s.nbi[3].p16x16_mv[1]; k++; }
+    if (c.nb & NB_TOP) { mvc[k][0] = s.nbi[1].p16x16_mv[0]; mvc[k][1] = s.nbi[1].p16x16_mv[1]; k++; }
+    if (c.p.ref_is_p) {
+      if (c.mbx < mbw - 1) { mvc[k][0] = c.f.ref_info[idx + 1].mv16[0]; mvc[k][1] = c.f.ref_info[idx + 1].mv16[1]; k++; }
+      if (c.mby < c.p.mb_h - 1) { mvc[k][0] = c.f.ref_info[idx + mbw].mv16[0]; mvc[k][1] = c.f.ref_info[idx + mbw].mv16[1]; k++; }
+    }
+  }
+  warp_sync();
+  win_wait(c, s);
   int plan[3] = {0, 0, 0}, n_plan = 0, cost = 0;       // shapes: 0 = 16x16, 1 = 16x8, 2 = 8x16, 3 = 8x8
   MBK_NO_UNROLL
   for (int t = -1; t < n_plan; t++) {
     const int shape = t < 0 ? 0 : plan[t];
     int cst = 0;
-    if (t >= 0 || !is_skip) {
-      const int np = shape == 0 ? 1 : shape == 3 ? 4 : 2;
-      MeState* arr = shape == 0 ? &me16 : shape == 1 ? me16x8 : shape == 2 ? me8x16 : me8x8;
-      MBK_NO_UNROLL
-      for (int i = 0; i < np; i++) {
-        int px = px16, py = py16, ox = 0, oy = 0, blk = BLK_16x16, ci = 0, cw = 4, ch = 4, ncand = n16;
-        uint32_t sp = (uint32_t)sad_pred_mb;
-        if (shape == 1) { pred_16x8_mv(s, 8 * i, 0, &px, &py); oy = 8 * i; blk = BLK_16x8; ci = 8 * i; ch = 2; sp = (uint32_t)(sad_pred_mb >> 1); ncand = 1; }
-        else if (shape == 2) { pred_8x16_mv(s, 4 * i, 0, &px, &py); ox = 8 * i; blk = BLK_8x16; ci = 4 * i; cw = 2; sp = (uint32_t)(sad_pred_mb >> 1); ncand = 1; }
-        else if (shape == 3) { pred_mv(s, 4 * i, 2, 0, &px, &py); ox = (i & 1) * 8; oy = (i >> 1) * 8; blk = BLK_8x8; ci = 4 * i; cw = 2; ch = 2; sp = (uint32_t)(sad_pred_mb >> 2); ncand = 1; }
-        me_partition(c, s, blk, ox, oy, px, py, sp, ncand, &mvc[0][0], &arr[i]);     // sub-partitions: candidate [0] = (0, 0) only
-        if (shape != 0) cache_set(s, ci, cw, ch, arr[i].mv_x, arr[i].mv_y);
-        cst += (int)arr[i].satd_cost;
-      }
+    const int np = shape == 0 ? 1 : shape == 3 ? 4 : 2;
+    MeState* arr = shape == 0 ? &me16 : shape == 1 ? me16x8 : shape == 2 ? me8x16 : me8x8;
+    MBK_NO_UNROLL
+    for (int i = 0; i < np; i++) {
+      int px = px16, py = py16, ox = 0, oy = 0, blk = BLK_16x16, ci = 0, cw = 4, ch = 4, ncand = n16;
+      uint32_t sp = (uint32_t)sad_pred_mb;
+      if (shape == 1) { pred_16x8_mv(s, 8 * i, 0, &px, &py); oy = 8 * i; blk = BLK_16x8; ci = 8 * i; ch = 2; sp = (uint32_t)(sad_pred_mb >> 1); ncand = 1; }
+      else if (shape == 2) { pred_8x16_mv(s, 4 * i, 0, &px, &py); ox = 8 * i; blk = BLK_8x16; ci = 4 * i; cw = 2; sp = (uint32_t)(sad_pred_mb >> 1); ncand = 1; }
+      else if (shape == 3) { pred_mv(s, 4 * i, 2, 0, &px, &py); ox = (i & 1) * 8; oy = (i >> 1) * 8; blk = BLK_8x8; ci = 4 * i; cw = 2; ch = 2; sp = (uint32_t)(sad_pred_mb >> 2); ncand = 1; }
+      me_partition(c, s, blk, ox, oy, px, py, sp, ncand, &mvc[0][0], &arr[i]);       // sub-partitions: candidate [0] = (0, 0) only
+      if (shape != 0) cache_set(s, ci, cw, ch, arr[i].mv_x, arr[i].mv_y);
+      cst += (int)arr[i].satd_cost;
     }
     if (t >= 0) {
       // the first shape of the plan has to beat 16x16, a later one only the best so far (<=: md.cpp keeps the later shape on a tie)
@@ -1039,8 +1058,8 @@ MBK_STAGE int inter_stage_b(const MbCtx& c, MbScratch& s) {
       continue;
     }
     // ---- after the 16x16 round ----
-    if (!is_skip) { p16_mvx = me16.mv_x; p16_mvy = me16.mv_y; cost_luma = cst; }
-    if (!is_skip) mbk_batch_sync(2, c.batch_n);                         // list B: together again after the 16x16 search
+    p16_mvx = me16.mv_x; p16_mvy = me16.mv_y; cost_luma = cst;
+    mbk_batch_sync(2, c.batch_n);                                          // list B: together again after the 16x16 search
     phase_mark(s, 3);
     {
       // intra check (WelsMdFirstIntraMode :1829)
@@ -1048,18 +1067,12 @@ MBK_STAGE int inter_stage_b(const MbCtx& c, MbScratch& s) {
       const int cost16 = md_i16x16_inl(c, s, &bb);
       phase_mark(s, 4);
       if (cost16 < cost_luma) {
-        st_save(s, is_skip ? 1 : 0, cost_luma, cost_skip_mb, p16_mvx, p16_mvy, final_type);
+        st_save(s, 0, cost_luma, cost_skip_mb, p16_mvx, p16_mvy, final_type);
         if (lane_id() == 0) { s.st.cost16 = cost16; s.st.bb = bb; }
         warp_sync();
-        if (!is_skip) { mbk_batch_leave(3, c.batch_n); mbk_batch_leave(4, c.batch_n); }
+        mbk_batch_leave(3, c.batch_n); mbk_batch_leave(4, c.batch_n);
         return MBS_C;
       }
-    }
-    if (is_skip) {
-      decided_pskip(c, s);
-      st_save(s, 1, cost_luma, cost_skip_mb, p16_mvx, p16_mvy, MBT_PSKIP);
-      inter_tail(c, s);
-      return MBS_DONE;
     }
     // LOW_COMPLEXITY: the four 8x8 SADs of the macroblock against the previous source picture say which partition shapes
     // are worth a search (MdInterAnalysisVaaInfo_c md.cpp:389): 15 = homogeneous, none; 3/12 -> 16x8; 5/10 -> 8x16;

@@ -34,13 +34,13 @@ __constant__ uint8_t c_tc0[52][3];
 #define DEC_WPC 24         // warps per CTA of the decoder's macroblock kernel (one CTA per SM at 80 registers)
 #define ENC_WPC 23         // WORKER warps per CTA of the encode kernel; one more warp schedules (24 x 32 x 80 registers = one CTA per SM)
 // A full batch of a PULLED list claims up to ENC_PULL x ENC_WPC tasks; a warp that finishes its task takes the next unstarted
-// one of the block (run_stages).  Pulled: A (skip test) and Bs (skip-candidate intra check), bit (stage - 1) of the mask.
+// one of the block (run_stages).  Pulled: A (skip test), bit enc_list(stage) of the mask.
 // ENC_PULL = 1 is the plain one-task-per-warp batch.
 #ifndef ENC_PULL
 #define ENC_PULL 2
 #endif
 #ifndef ENC_PULL_LISTS
-#define ENC_PULL_LISTS ((1 << (MBS_A - 1)) | (1 << (MBS_BSKIP - 1)))
+#define ENC_PULL_LISTS (1 << enc_list(MBS_A))
 #endif
 
 __device__ __forceinline__ int ld_volatile(const int* p) { return *reinterpret_cast<const volatile int*>(p); }
@@ -98,7 +98,11 @@ __global__ void __launch_bounds__(256) k_vaa_sad8x8(const StreamFrame* __restric
 // neighbour; the second notification pushes the MB onto a global ready list.  Persistent warps pop the
 // list: no warp ever holds an SM slot while a row it depends on is still busy (a row-per-warp wavefront
 // spent most of its issue slots spinning).  The encoder has one ready list per stage (below), the decoder one list.
-enum { NQ = MBS_COUNT - 1 };                       // the encoder's ready lists, index = stage - 1
+// the encoder's ready lists: one per stage (MBP_SKIPCAND_INTRA is not a stage), index enc_list(stage)
+enum { NQ = MBS_COUNT - 2 };
+__host__ __device__ constexpr int enc_list(int stage) { return stage < MBP_SKIPCAND_INTRA ? stage - 1 : stage - 2; }
+__host__ __device__ constexpr int enc_stage(int list) { return list < MBP_SKIPCAND_INTRA - 1 ? list + 1 : list + 2; }
+static_assert(enc_stage(enc_list(MBS_C)) == MBS_C && enc_list(MBS_C) == NQ - 1, "one list per stage");
 struct MbSched {
   int* dep;          // per (stream, mb): notifications received so far
   int* queue;        // ready lists of capacity `total` each, -1 = slot not yet written
@@ -163,13 +167,12 @@ __device__ __forceinline__ void run_mbs(const StreamFrame* sf, int n_streams, co
 // its own ready list, and a batch comes from ONE list.  A macroblock that needs another stage parks its scratch in
 // global memory (one slot per stream and macroblock ROW: at most one macroblock of a row is in flight) and is
 // pushed onto the next stage's list; whichever CTA takes it continues from the parked scratch.
-// Only the live part of a scratch is parked (enc_mb.cuh: kParkCore + skip_pred or pred_y): slot = kParkSlot bytes
+// Only the live part of a scratch is parked (enc_mb.cuh: kParkCore, + pred_y for stage C): slot = kParkSlot bytes
 constexpr int kStashU4 = kParkSlot / 16, kCoreU4 = kParkCore / 16;
 static_assert(kParkSlot % 16 == 0 && kParkCore % 16 == 0, "parked ranges are copied as uint4");
 // second parked range of a macroblock that continues at `stage`: offset (uint4 units) and length
 __device__ __forceinline__ void park_extra(int stage, int* off, int* n) {
-  if (stage == MBS_BSKIP) { *off = (int)(offsetof(MbScratch, skip_pred) / 16); *n = 384 / 16; }
-  else if (stage == MBS_C) { *off = (int)(offsetof(MbScratch, pred_y) / 16); *n = 512 / 16; }
+  if (stage == MBS_C) { *off = (int)(offsetof(MbScratch, pred_y) / 16); *n = 512 / 16; }
   else { *off = 0; *n = 0; }
 }
 
@@ -221,7 +224,7 @@ __device__ __forceinline__ void run_task(const StreamFrame* sf, const MbSched& q
   if (next == MBS_DONE) {
     __threadfence();
     if (lane == 0) {
-      notify_dependants(q, total, (sf[si].p.is_idr ? MBS_I : MBS_A) - 1, id, x, y, mb_w, mb_h);
+      notify_dependants(q, total, enc_list(sf[si].p.is_idr ? MBS_I : MBS_A), id, x, y, mb_w, mb_h);
       atomicAdd(ctl_done(q), 1);
     }
   } else {
@@ -230,7 +233,7 @@ __device__ __forceinline__ void run_task(const StreamFrame* sf, const MbSched& q
     for (int i = lane; i < kCoreU4 + xn; i += 32) park[i] = i < kCoreU4 ? sc[i] : sc[xo + i - kCoreU4];
     __threadfence();
     __syncwarp();
-    if (lane == 0) ready_push(q, total, next - 1, id);
+    if (lane == 0) ready_push(q, total, enc_list(next), id);
   }
 }
 
@@ -242,13 +245,13 @@ __device__ __forceinline__ void run_task(const StreamFrame* sf, const MbSched& q
 // the list holds two batches' worth); a partial batch only when the workers are already waiting — exactly the decision
 // thread 0 used to take at that moment.  (Experiments that gave up the common start of a batch — warp-asynchronous
 // draws, 2 x 12 and 3 x 8 warp groups — lost more than they saved to instruction-cache misses.)
-// The short stages (A, Bs: ENC_PULL_LISTS) paid the batch barrier, the claim and the slowest warp once per ENC_WPC tasks of
+// The short stage (A: ENC_PULL_LISTS) paid the batch barrier, the claim and the slowest warp once per ENC_WPC tasks of
 // ~20 k cycles each.  A full batch of such a list claims up to ENC_PULL x ENC_WPC tasks: every warp starts on task `warp`
 // together as before, then takes the next unstarted task of the block (a shared counter per slot) until the block is
 // empty; the warps drift apart inside the stage, which costs nothing measurable there (DESIGN.md §2).  "The first worker
 // has finished" becomes "a worker found the block empty" (counter > n).  List B stays one task per warp: its
 // re-alignment points (mbk_batch_sync) count the batch's warps.
-static_assert(!(ENC_PULL_LISTS & (1 << (MBS_B - 1))), "stage B's re-alignment barriers need one task per warp");
+static_assert(!(ENC_PULL_LISTS & (1 << enc_list(MBS_B))), "stage B's re-alignment barriers need one task per warp");
 static_assert(ENC_PULL >= 1, "a pulled batch holds up to ENC_PULL x ENC_WPC tasks");
 struct BatchSlot { int k, base, n, pad; };
 constexpr int kEncThreads = 32 * (ENC_WPC + 1);
@@ -370,7 +373,7 @@ __device__ __forceinline__ void run_stages(const StreamFrame* sf, int n_streams,
     const int k = s_slot[p].k, n = s_slot[p].n;
     if (t < n) {
       const long long t_task = stats ? clock64() : 0;
-      run_task(sf, q, s, s_ids[p][t], k + 1, mb_w, mb_h, total, min(n, ENC_WPC) /* batch_n: warps, not tasks */, body);
+      run_task(sf, q, s, s_ids[p][t], enc_stage(k), mb_w, mb_h, total, min(n, ENC_WPC) /* batch_n: warps, not tasks */, body);
       const int kt = ld_volatile(&s_slot[p].k), nt = ld_volatile(&s_slot[p].n);
       if (lane == 0) atomicAdd(&s_fin[p], 1);
       if (stats && lane == 0) { atomicAdd(&g_task_wall[kt][0], (unsigned long long)(clock64() - t_task)); atomicAdd(&g_task_wall[kt][1], 1ull); }
@@ -388,18 +391,18 @@ __device__ __forceinline__ void run_stages(const StreamFrame* sf, int n_streams,
 
 // MB (0,0) of every stream is ready.  The encoder (n_lists = NQ) puts IDR pictures on list I and P pictures on list A, the
 // decoder (n_lists = 1) every stream on list 0, which is list A's index.
-static_assert(MBS_A - 1 == 0, "list 0 is list A");
+static_assert(enc_list(MBS_A) == 0, "list 0 is list A");
 __global__ void k_ready_init(MbSched q, const StreamFrame* __restrict__ sf, int n_streams, int n_mb, int n_lists) {
   if (threadIdx.x != 0) return;
   int na = 0, ni = 0;
   const int total = n_streams * n_mb;
   for (int s = 0; s < n_streams; s++) {
-    if (n_lists > 1 && sf[s].p.is_idr) q.queue[(size_t)(MBS_I - 1) * total + ni++] = s * n_mb;
-    else q.queue[(size_t)(MBS_A - 1) * total + na++] = s * n_mb;
+    if (n_lists > 1 && sf[s].p.is_idr) q.queue[(size_t)enc_list(MBS_I) * total + ni++] = s * n_mb;
+    else q.queue[(size_t)enc_list(MBS_A) * total + na++] = s * n_mb;
   }
   for (int k = 0; k < 32 * (n_lists + 1); k++) q.ctl[k] = 0;
-  *ctl_tail(q, MBS_A - 1) = na;
-  if (n_lists > 1) *ctl_tail(q, MBS_I - 1) = ni;
+  *ctl_tail(q, enc_list(MBS_A)) = na;
+  if (n_lists > 1) *ctl_tail(q, enc_list(MBS_I)) = ni;
 }
 
 // optional per-MB-type cycle statistics (debug): [type*2] = cycles, [type*2+1] = count

@@ -48,7 +48,7 @@ enum { WIN_W = 64, WIN_H = 48 };
 
 // Per-warp working set (shared memory on the device, a plain struct in the host emulation build).
 // Plain data only: the device scheduler parks the LIVE PART in global memory between stages — the prefix up to
-// and including the header of `out` (kParkCore) plus, per transition, skip_pred (A -> Bs) or pred_y (B -> C);
+// and including the header of `out` (kParkCore) plus pred_y when the macroblock goes on to stage C;
 // everything behind is dead across a stage boundary (cur_y / cur_c are re-read from the source picture).
 struct alignas(128) MbScratch {
   // ---- parked prefix -------------------------------------------------------------------------------------
@@ -65,7 +65,7 @@ struct alignas(128) MbScratch {
   int32_t nb_sad[4];            // neighbours' persistent SAD cost (pSadCost[0])
   int32_t nb_skip_sad[4];       // neighbours' skip SAD of THIS picture (pMbSkipSad)
   alignas(16) MbOut out;        // staged output record: the header (MBOUT_HEADER_WORDS) is live, the levels are not
-  // ---- not parked (except skip_pred / pred_y, see above) ------------------------------------------------------
+  // ---- not parked (except pred_y, see above) -----------------------------------------------------------------
   alignas(16) uint8_t pred_y[2][256];       // luma prediction ping-pong (pMemPredMb)
   // The next four are contiguous and double as the search window (3072 of their 3136 bytes, 128-byte aligned for
   // the bulk tensor copy): the window lives from the start of stage B's 16x16 search to the last sub-partition
@@ -96,7 +96,7 @@ static_assert(offsetof(MbScratch, pred_c) % 128 == 0 && offsetof(MbScratch, skip
               offsetof(MbScratch, out) % 16 == 0, "alignment of the parked ranges / the bulk copy destination");
 // bytes of the scratch that cross every stage boundary
 constexpr int kParkCore = (int)((offsetof(MbScratch, out) + 4 * MBOUT_HEADER_WORDS + 15) / 16 * 16);
-constexpr int kParkExtra = 512;                               // skip_pred (384) or pred_y (512)
+constexpr int kParkExtra = 512;                               // pred_y (A or B -> C)
 constexpr int kParkSlot = kParkCore + kParkExtra;
 MBK_HD uint8_t* scratch_win(MbScratch& s) { return &s.pred_c[0][0]; }
 
@@ -400,7 +400,8 @@ MBK_HD int md_i16x16_inl(const MbCtx& c, MbScratch& s, int* best_buf) {
   *best_buf = 0;
   return best;
 }
-// the shared (real-call) copy of the intra paths; stage B / Bs of a P picture, which runs it for every non-skipped macroblock, inlines it
+// the shared (real-call) copy of the intra paths; stages A and B of a P picture, which run it for every skip candidate and every
+// macroblock they search, inline it
 MBK_FN int md_i16x16(const MbCtx& c, MbScratch& s, int* best_buf) { return md_i16x16_inl(c, s, best_buf); }
 
 // ---- intra chroma mode decision (WelsMdIntraChroma, :867) ---------------------------------------
