@@ -15,12 +15,14 @@
 #include <string.h>
 
 #include <chrono>
+#include <memory>
 #include <type_traits>
 
 #include <vector>
 
 #include "../../include/b2h264_codec.h"
 #include "b2h264_internal.h"
+#include "cuda_owned.h"
 #include "enc_host.h"
 #include "enc_launch.h"
 #include "h264_parse.h"
@@ -38,46 +40,43 @@ struct DecOutPic {                        // b2h264_dec_decode_device: one activ
 struct b2h264_dec {
   b2h264_dec_config cfg;
   int S = 0, mb_w = 0, mb_h = 0, n_mb = 0;
-  StreamCtl geo;                          // picture geometry (strides, padded rows)
+  PicLayout lay;                          // of each picture slot; pic_bytes = lay.bytes() is the slot pitch
   std::vector<ParserState> parser;
   std::vector<ParsedPicture> parsed;      // per stream: the access unit of the running call
   std::vector<int> parse_rc;
-  Pool* pool = nullptr;                   // the streams are parsed side by side (the parser is the decoder's host cost)
   int slots = 2;                          // picture slots per stream (num_ref_frames + 1 of the most demanding stream so far)
   std::vector<int> out_cx, out_cy;        // per active stream: luma samples cropped at the left / top of the output
   std::vector<int> out_slot;              // per active stream: slot of the picture decoded in this call
   std::vector<int> act;
   std::vector<uint8_t> act_ref;           // is the picture of act[i] a reference picture
-  cudaStream_t st = nullptr;
-  bool own_stream = true;                 // false after b2h264_dec_set_stream: the caller's stream is not destroyed here
-  cudaEvent_t staged = nullptr;           // after the last host-to-device copy of a call: the pinned buffers may be rewritten
-  uint8_t* d_pic = nullptr;               // S x slots padded pictures: picture (s, slot) at (s * slots + slot) * pic_bytes
-  MbInfo* d_mbi = nullptr;
-  MbOut* d_recs = nullptr;
-  MbOut* h_recs = nullptr;                // pinned: COMPACT records (pack_records_compact), one worst-case slot per stream
-  uint8_t* d_pack = nullptr;              // device copy of the compact records (same slots)
-  int32_t* h_idx = nullptr;               // pinned: per macroblock offset of its compact record or -1 - qp (skipped)
-  int32_t* d_idx = nullptr;
+  // the CUDA resources are released in the reverse order of their declaration: the buffers and the event before the stream
+  Stream own_st;                          // the decoder's stream until b2h264_dec_set_stream lends it the caller's
+  cudaStream_t st = nullptr;              // own_st or the caller's stream
+  Event staged;                           // after the last host-to-device copy of a call: the pinned buffers may be rewritten
+  DeviceBuf<uint8_t> d_pic;               // S x slots padded pictures: picture (s, slot) at (s * slots + slot) * pic_bytes
+  DeviceBuf<MbInfo> d_mbi;
+  DeviceBuf<MbOut> d_recs;
+  HostBuf<MbOut> h_recs;                  // pinned: COMPACT records (pack_records_compact), one worst-case slot per stream
+  DeviceBuf<uint8_t> d_pack;              // device copy of the compact records (same slots)
+  HostBuf<int32_t> h_idx;                 // pinned: per macroblock offset of its compact record or -1 - qp (skipped)
+  DeviceBuf<int32_t> d_idx;
   std::vector<int> units;                 // 32-byte units packed per active stream
-  DecMbAux* d_aux = nullptr;
-  DecMbAux* h_aux = nullptr;              // pinned
-  DecMbAuxB* d_aux_b = nullptr;           // list 1 of B macroblocks: allocated when the first picture with B slices arrives
-  DecMbAuxB* h_aux_b = nullptr;           // pinned
+  DeviceBuf<DecMbAux> d_aux;
+  HostBuf<DecMbAux> h_aux;                // pinned
+  DeviceBuf<DecMbAuxB> d_aux_b;           // list 1 of B macroblocks: allocated when the first picture with B slices arrives
+  HostBuf<DecMbAuxB> h_aux_b;             // pinned
   std::vector<int> last_poc, last_idr, last_reorder;   // per stream: picture order count / IDR flag / reorder depth of the last decoded picture
-  StreamFrame* d_sf = nullptr;
-  StreamFrame* h_sf = nullptr;            // pinned
-  DecOutPic* d_out = nullptr;             // device output: per active stream, the sources and the destination of its planes
-  DecOutPic* h_out = nullptr;             // pinned
-  int* d_ws = nullptr;
-  size_t pic_bytes = 0, pic_y_bytes = 0, pic_c_bytes = 0;
+  DeviceBuf<StreamFrame> d_sf;
+  HostBuf<StreamFrame> h_sf;              // pinned
+  DeviceBuf<DecOutPic> d_out;             // device output: per active stream, the sources and the destination of its planes
+  HostBuf<DecOutPic> h_out;               // pinned
+  DeviceBuf<int> d_ws;
+  size_t pic_bytes = 0;
   int last_error_stream = -1;
+  std::unique_ptr<Pool> pool;             // the streams are parsed side by side (the parser is the decoder's host cost); declared
+                                          // last: its threads stop before anything else is released
 
-  uint8_t* plane0(int slot, int s, int pl) const {
-    const int sty = geo.rec_stride_y(), stc = geo.rec_stride_c();
-    uint8_t* base = d_pic + ((size_t)s * slots + slot) * pic_bytes;
-    if (pl == 0) return base + (size_t)32 * sty + 32;
-    return base + pic_y_bytes + (size_t)(pl - 1) * pic_c_bytes + (size_t)16 * stc + 16;
-  }
+  uint8_t* plane0(int slot, int s, int pl) const { return d_pic.get() + ((size_t)s * slots + slot) * pic_bytes + lay.plane0(pl); }
 };
 
 // ---- device output: the cropped pictures of one call into the caller's HBM, every active stream and plane in one launch ----
@@ -117,62 +116,58 @@ __global__ void __launch_bounds__(256) k_dec_output(const DecOutPic* __restrict_
 
 extern "C" {
 
-int b2h264_dec_create(const b2h264_dec_config* cfg, b2h264_dec** out) {
-  if (!cfg || !out) return -1;
+static int dec_create(const b2h264_dec_config* cfg, b2h264_dec** out) {
   if (cfg->width < 16 || cfg->height < 16 || (cfg->width & 1) || (cfg->height & 1) || cfg->n_streams < 1) return -2;
   int rc = b2h264_init(cfg->device);
   if (rc) return rc;
   if ((rc = enc_upload_deblock_tables())) return rc;
-  b2h264_dec* d = new b2h264_dec();
+  std::unique_ptr<b2h264_dec> d(new b2h264_dec());
   d->cfg = *cfg;
   d->S = cfg->n_streams;
-  d->geo.init(cfg->width, cfg->height, 26, 30.0f, 0);
-  d->mb_w = d->geo.sp.mb_w; d->mb_h = d->geo.sp.mb_h; d->n_mb = d->mb_w * d->mb_h;
+  d->mb_w = (cfg->width + 15) >> 4; d->mb_h = (cfg->height + 15) >> 4; d->n_mb = d->mb_w * d->mb_h;
   d->parser.resize(d->S);
   d->parsed.resize(d->S);
   d->parse_rc.assign(d->S, 0);
-  { int nt = usable_cores(); if (nt > d->S) nt = d->S; d->pool = new Pool(nt < 1 ? 1 : nt); }
-  d->pic_y_bytes = (size_t)d->geo.rec_stride_y() * d->geo.rec_rows_y();
-  d->pic_c_bytes = (size_t)d->geo.rec_stride_c() * d->geo.rec_rows_c();
-  d->pic_bytes = d->pic_y_bytes + 2 * d->pic_c_bytes;
+  d->lay = PicLayout(d->mb_w, d->mb_h);
+  d->pic_bytes = d->lay.bytes();
   const size_t S = d->S;
-  CK(cudaStreamCreateWithFlags(&d->st, cudaStreamNonBlocking));
-  CK(cudaMalloc(&d->d_pic, S * d->slots * d->pic_bytes + 256));
-  CK(cudaMemset(d->d_pic, 0, S * d->slots * d->pic_bytes + 256));
-  CK(cudaMalloc(&d->d_mbi, S * d->n_mb * sizeof(MbInfo)));
-  CK(cudaMemset(d->d_mbi, 0, S * d->n_mb * sizeof(MbInfo)));
-  CK(cudaMalloc(&d->d_recs, S * d->n_mb * sizeof(MbOut)));
-  CK(cudaMallocHost(&d->h_recs, S * d->n_mb * sizeof(MbOut)));
-  CK(cudaMalloc(&d->d_pack, S * d->n_mb * sizeof(MbOut)));
-  CK(cudaMallocHost(&d->h_idx, S * d->n_mb * sizeof(int32_t)));
-  CK(cudaMalloc(&d->d_idx, S * d->n_mb * sizeof(int32_t)));
+  CK(d->own_st.create(cudaStreamNonBlocking));
+  d->st = d->own_st.get();
+  CK(d->d_pic.alloc(S * d->slots * d->pic_bytes + 256));
+  CK(cudaMemset(d->d_pic.get(), 0, S * d->slots * d->pic_bytes + 256));
+  CK(d->d_mbi.alloc(S * d->n_mb * sizeof(MbInfo)));
+  CK(cudaMemset(d->d_mbi.get(), 0, S * d->n_mb * sizeof(MbInfo)));
+  CK(d->d_recs.alloc(S * d->n_mb * sizeof(MbOut)));
+  CK(d->h_recs.alloc(S * d->n_mb * sizeof(MbOut)));
+  CK(d->d_pack.alloc(S * d->n_mb * sizeof(MbOut)));
+  CK(d->h_idx.alloc(S * d->n_mb * sizeof(int32_t)));
+  CK(d->d_idx.alloc(S * d->n_mb * sizeof(int32_t)));
   d->units.assign(d->S, 0);
   d->last_poc.assign(d->S, 0); d->last_idr.assign(d->S, 0); d->last_reorder.assign(d->S, 0);
-  CK(cudaMalloc(&d->d_aux, S * d->n_mb * sizeof(DecMbAux)));
-  CK(cudaMallocHost(&d->h_aux, S * d->n_mb * sizeof(DecMbAux)));
-  CK(cudaMalloc(&d->d_sf, S * sizeof(StreamFrame)));
-  CK(cudaMallocHost(&d->h_sf, S * sizeof(StreamFrame)));
-  CK(cudaMalloc(&d->d_out, S * sizeof(DecOutPic)));
-  CK(cudaMallocHost(&d->h_out, S * sizeof(DecOutPic)));
-  CK(cudaEventCreateWithFlags(&d->staged, cudaEventDisableTiming));
-  CK(cudaMalloc(&d->d_ws, dec_sched_ints((int)S, d->mb_w, d->mb_h) * sizeof(int)));
-  *out = d;
+  CK(d->d_aux.alloc(S * d->n_mb * sizeof(DecMbAux)));
+  CK(d->h_aux.alloc(S * d->n_mb * sizeof(DecMbAux)));
+  CK(d->d_sf.alloc(S * sizeof(StreamFrame)));
+  CK(d->h_sf.alloc(S * sizeof(StreamFrame)));
+  CK(d->d_out.alloc(S * sizeof(DecOutPic)));
+  CK(d->h_out.alloc(S * sizeof(DecOutPic)));
+  CK(d->staged.create(cudaEventDisableTiming));
+  CK(d->d_ws.alloc(dec_sched_ints((int)S, d->mb_w, d->mb_h) * sizeof(int)));
+  { int nt = usable_cores(); if (nt > d->S) nt = d->S; d->pool.reset(new Pool(nt < 1 ? 1 : nt)); }
+  *out = d.release();
   return 0;
+}
+
+int b2h264_dec_create(const b2h264_dec_config* cfg, b2h264_dec** out) {
+  if (!cfg || !out) return -1;
+  const int rc = dec_create(cfg, out);
+  if (rc > 0) (void)cudaGetLastError();    // the failure is returned here: later launch checks must not see it
+  return rc;
 }
 
 void b2h264_dec_destroy(b2h264_dec* d) {
   if (!d) return;
   cudaSetDevice(d->cfg.device);
-  if (d->st) cudaStreamSynchronize(d->st);
-  cudaFree(d->d_pic);
-  cudaFree(d->d_mbi); cudaFree(d->d_recs); cudaFree(d->d_aux); cudaFreeHost(d->h_aux); cudaFree(d->d_sf); cudaFree(d->d_ws);
-  if (d->d_aux_b) cudaFree(d->d_aux_b);
-  if (d->h_aux_b) cudaFreeHost(d->h_aux_b);
-  cudaFreeHost(d->h_recs); cudaFreeHost(d->h_sf); cudaFree(d->d_pack); cudaFreeHost(d->h_idx); cudaFree(d->d_idx);
-  cudaFree(d->d_out); cudaFreeHost(d->h_out);
-  if (d->staged) cudaEventDestroy(d->staged);
-  if (d->st && d->own_stream) cudaStreamDestroy(d->st);
-  delete d->pool;
+  cudaStreamSynchronize(d->st);
   delete d;
 }
 
@@ -201,7 +196,7 @@ static int dec_decode_impl(b2h264_dec* d, const uint8_t* const* au, const int32_
   }
   const double t_parse = ms_since(t0);
   // the pinned staging buffers still feed the previous call's copies until they are issued: the parse above overlapped them
-  CK(cudaEventSynchronize(d->staged));
+  CK(cudaEventSynchronize(d->staged.get()));
   // 2. the batch: descriptors and records of the streams that carry a picture, in stream order
 #define STREAM_FAIL(code) { d->last_error_stream = s; if (status) { status[s] = (code); continue; } return (code); }
   if (status) for (int s = 0; s < S; s++) status[s] = 0;
@@ -222,17 +217,16 @@ static int dec_decode_impl(b2h264_dec* d, const uint8_t* const* au, const int32_
     if (pic.has_b && (int)pic.aux_b.size() != d->n_mb) STREAM_FAIL(-103)
     if (pic.n_slots > d->slots) {                   // a stream with more reference frames: widen every stream's slot array, keeping the pictures
       if (pic.n_slots > 17) STREAM_FAIL(-103)
-      uint8_t* np = nullptr;
-      CK(cudaMalloc(&np, (size_t)S * pic.n_slots * d->pic_bytes + 256));
-      CK(cudaMemsetAsync(np, 0, (size_t)S * pic.n_slots * d->pic_bytes + 256, d->st));
+      DeviceBuf<uint8_t> np;
+      CK(np.alloc((size_t)S * pic.n_slots * d->pic_bytes + 256));
+      CK(cudaMemsetAsync(np.get(), 0, (size_t)S * pic.n_slots * d->pic_bytes + 256, d->st));
       for (int q = 0; q < S; q++)
-        CK(cudaMemcpyAsync(np + (size_t)q * pic.n_slots * d->pic_bytes, d->d_pic + (size_t)q * d->slots * d->pic_bytes,
+        CK(cudaMemcpyAsync(np.get() + (size_t)q * pic.n_slots * d->pic_bytes, d->d_pic.get() + (size_t)q * d->slots * d->pic_bytes,
                            (size_t)d->slots * d->pic_bytes, cudaMemcpyDeviceToDevice, d->st));
       CK(cudaStreamSynchronize(d->st));
-      cudaFree(d->d_pic);
-      d->d_pic = np; d->slots = pic.n_slots;
+      d->d_pic = std::move(np); d->slots = pic.n_slots;
       for (int q = 0; q < (int)d->act.size(); q++) {      // descriptors built before the move
-        StreamFrame& G = d->h_sf[q];
+        StreamFrame& G = d->h_sf.get()[q];
         const int qs = d->act[q];
         for (int pl = 0; pl < 3; pl++) { G.f.rec[pl] = d->plane0(d->out_slot[q], qs, pl); G.f.ref[pl] = G.f.dpb0[pl] = d->plane0(0, qs, pl); }
       }
@@ -241,23 +235,26 @@ static int dec_decode_impl(b2h264_dec* d, const uint8_t* const* au, const int32_
     if (pic.any_deblock) deblock = 1;               // the filter kernel runs if any slice of any stream wants it (per-MB control inside)
     const int i = (int)d->act.size();
     d->act.push_back(s); d->act_ref.push_back(pic.is_ref ? 1 : 0); d->out_slot.push_back(pic.cur_slot); d->out_cx.push_back(pic.crop_left); d->out_cy.push_back(pic.crop_top);
-    StreamFrame& F = d->h_sf[i];
+    StreamFrame& F = d->h_sf.get()[i];
     memset(&F, 0, sizeof(F));
     F.p.mb_w = d->mb_w; F.p.mb_h = d->mb_h;
-    F.p.rec_stride_y = d->geo.rec_stride_y(); F.p.rec_stride_c = d->geo.rec_stride_c();
+    F.p.rec_stride_y = d->lay.stride_y; F.p.rec_stride_c = d->lay.stride_c;
     F.p.dec_cqp_off = pic.chroma_qp_offset;
     F.p.qp = pic.ss.qp; F.p.is_idr = pic.ss.idr; F.p.ref_is_p = !pic.ss.idr; F.p.mv_range = 64; F.p.dec_mode = 1;
     if (pic.cur_slot >= d->slots) STREAM_FAIL(-103)
     for (int pl = 0; pl < 3; pl++) { F.f.rec[pl] = d->plane0(pic.cur_slot, s, pl); F.f.ref[pl] = F.f.dpb0[pl] = d->plane0(0, s, pl); }
     F.f.dpb_stride = (int64_t)d->pic_bytes;
-    F.f.mbi = d->d_mbi + (size_t)s * d->n_mb;
+    F.f.mbi = d->d_mbi.get() + (size_t)s * d->n_mb;
     d->last_poc[s] = pic.poc; d->last_idr[s] = (pic.ss.idr ? 1 : 0) | (pic.has_b ? 2 : 0); d->last_reorder[s] = pic.max_reorder;
     if (pic.has_b) {                                // list-1 records of the picture's B macroblocks travel beside the aux records
-      if (!d->d_aux_b) {
-        CK(cudaMalloc(&d->d_aux_b, (size_t)S * d->n_mb * sizeof(DecMbAuxB)));
-        CK(cudaMallocHost(&d->h_aux_b, (size_t)S * d->n_mb * sizeof(DecMbAuxB)));
+      if (!d->d_aux_b.get()) {
+        DeviceBuf<DecMbAuxB> db;
+        HostBuf<DecMbAuxB> hb;
+        CK(db.alloc((size_t)S * d->n_mb * sizeof(DecMbAuxB)));
+        CK(hb.alloc((size_t)S * d->n_mb * sizeof(DecMbAuxB)));
+        d->d_aux_b = std::move(db); d->h_aux_b = std::move(hb);
       }
-      F.f.dec_aux_b = d->d_aux_b + (size_t)i * d->n_mb;
+      F.f.dec_aux_b = d->d_aux_b.get() + (size_t)i * d->n_mb;
     }
   }
   const int n = (int)d->act.size();
@@ -265,45 +262,45 @@ static int dec_decode_impl(b2h264_dec* d, const uint8_t* const* au, const int32_
   {
     std::function<void(int)> job = [&](int i) {          // compact records + index table into the stream's pinned slot
       const ParsedPicture& pic = d->parsed[d->act[i]];
-      d->units[i] = pack_records_compact(pic.mbs.data(), d->n_mb, reinterpret_cast<uint8_t*>(d->h_recs + (size_t)i * d->n_mb), d->h_idx + (size_t)i * d->n_mb);
-      memcpy(d->h_aux + (size_t)i * d->n_mb, pic.aux.data(), (size_t)d->n_mb * sizeof(DecMbAux));
-      if (pic.has_b) memcpy(d->h_aux_b + (size_t)i * d->n_mb, pic.aux_b.data(), (size_t)d->n_mb * sizeof(DecMbAuxB));
+      d->units[i] = pack_records_compact(pic.mbs.data(), d->n_mb, reinterpret_cast<uint8_t*>(d->h_recs.get() + (size_t)i * d->n_mb), d->h_idx.get() + (size_t)i * d->n_mb);
+      memcpy(d->h_aux.get() + (size_t)i * d->n_mb, pic.aux.data(), (size_t)d->n_mb * sizeof(DecMbAux));
+      if (pic.has_b) memcpy(d->h_aux_b.get() + (size_t)i * d->n_mb, pic.aux_b.data(), (size_t)d->n_mb * sizeof(DecMbAuxB));
     };
     d->pool->run(n, job);
   }
   const double t_pack = ms_since(t0);
   for (int i = 0; i < n; i++)                            // only what was packed crosses PCIe
     if (d->units[i] > 0)
-      CK(cudaMemcpyAsync(d->d_pack + (size_t)i * d->n_mb * sizeof(MbOut), d->h_recs + (size_t)i * d->n_mb, (size_t)d->units[i] * 32, cudaMemcpyHostToDevice, d->st));
-  CK(cudaMemcpyAsync(d->d_idx, d->h_idx, (size_t)n * d->n_mb * sizeof(int32_t), cudaMemcpyHostToDevice, d->st));
-  { const int rcu = dec_launch_unpack(d->d_pack, (size_t)d->n_mb * sizeof(MbOut), d->d_idx, d->d_recs, n, d->n_mb, d->st); if (rcu) return rcu; }
-  CK(cudaMemcpyAsync(d->d_aux, d->h_aux, (size_t)n * d->n_mb * sizeof(DecMbAux), cudaMemcpyHostToDevice, d->st));
+      CK(cudaMemcpyAsync(d->d_pack.get() + (size_t)i * d->n_mb * sizeof(MbOut), d->h_recs.get() + (size_t)i * d->n_mb, (size_t)d->units[i] * 32, cudaMemcpyHostToDevice, d->st));
+  CK(cudaMemcpyAsync(d->d_idx.get(), d->h_idx.get(), (size_t)n * d->n_mb * sizeof(int32_t), cudaMemcpyHostToDevice, d->st));
+  { const int rcu = dec_launch_unpack(d->d_pack.get(), (size_t)d->n_mb * sizeof(MbOut), d->d_idx.get(), d->d_recs.get(), n, d->n_mb, d->st); if (rcu) return rcu; }
+  CK(cudaMemcpyAsync(d->d_aux.get(), d->h_aux.get(), (size_t)n * d->n_mb * sizeof(DecMbAux), cudaMemcpyHostToDevice, d->st));
   for (int i = 0; i < n; i++)
     if (d->parsed[d->act[i]].has_b)
-      CK(cudaMemcpyAsync(d->d_aux_b + (size_t)i * d->n_mb, d->h_aux_b + (size_t)i * d->n_mb, (size_t)d->n_mb * sizeof(DecMbAuxB), cudaMemcpyHostToDevice, d->st));
-  CK(cudaMemcpyAsync(d->d_sf, d->h_sf, (size_t)n * sizeof(StreamFrame), cudaMemcpyHostToDevice, d->st));
+      CK(cudaMemcpyAsync(d->d_aux_b.get() + (size_t)i * d->n_mb, d->h_aux_b.get() + (size_t)i * d->n_mb, (size_t)d->n_mb * sizeof(DecMbAuxB), cudaMemcpyHostToDevice, d->st));
+  CK(cudaMemcpyAsync(d->d_sf.get(), d->h_sf.get(), (size_t)n * sizeof(StreamFrame), cudaMemcpyHostToDevice, d->st));
   const int w = d->cfg.width, h = d->cfg.height;
   if (on_device) {
     for (int i = 0; i < n; i++) {
-      DecOutPic& O = d->h_out[i];
+      DecOutPic& O = d->h_out.get()[i];
       for (int pl = 0; pl < 3; pl++) {
         const int c = pl ? 1 : 0;
-        O.src[pl] = d->plane0(d->out_slot[i], d->act[i], pl) + (size_t)(d->out_cy[i] >> c) * (pl ? d->geo.rec_stride_c() : d->geo.rec_stride_y()) + (d->out_cx[i] >> c);
+        O.src[pl] = d->plane0(d->out_slot[i], d->act[i], pl) + (size_t)(d->out_cy[i] >> c) * d->lay.stride(pl) + (d->out_cx[i] >> c);
       }
       O.dst = yuv[d->act[i]];
     }
-    CK(cudaMemcpyAsync(d->d_out, d->h_out, (size_t)n * sizeof(DecOutPic), cudaMemcpyHostToDevice, d->st));
+    CK(cudaMemcpyAsync(d->d_out.get(), d->h_out.get(), (size_t)n * sizeof(DecOutPic), cudaMemcpyHostToDevice, d->st));
   }
-  CK(cudaEventRecord(d->staged, d->st));
+  CK(cudaEventRecord(d->staged.get(), d->st));
   int b_slices = 0;
   for (int i = 0; i < n; i++) b_slices |= (d->parsed[d->act[i]].has_b || d->parsed[d->act[i]].has_t8) ? 1 : 0;   // Main / High tools: the wider filter kernel
-  const int rc = dec_launch_frame(d->d_sf, n, d->mb_w, d->mb_h, d->d_ws, d->d_recs, d->d_aux, deblock, d->st, b_slices);
+  const int rc = dec_launch_frame(d->d_sf.get(), n, d->mb_w, d->mb_h, d->d_ws.get(), d->d_recs.get(), d->d_aux.get(), deblock, d->st, b_slices);
   if (rc) return rc;
   const double t_launch = ms_since(t0);
   if (timing) cudaStreamSynchronize(d->st);
   const double t_kernels = ms_since(t0);
   if (on_device) {
-    k_dec_output<<<dim3((2 * h + 7) / 8, n), 256, 0, d->st>>>(d->d_out, w, h, d->geo.rec_stride_y(), d->geo.rec_stride_c());
+    k_dec_output<<<dim3((2 * h + 7) / 8, n), 256, 0, d->st>>>(d->d_out.get(), w, h, d->lay.stride_y, d->lay.stride_c);
     const int rco = b2h264_launched();
     if (rco) return rco;
     for (int i = 0; i < n; i++) status[d->act[i]] = 1;
@@ -314,7 +311,7 @@ static int dec_decode_impl(b2h264_dec* d, const uint8_t* const* au, const int32_
     uint8_t* dst = yuv[s];
     for (int pl = 0; pl < 3; pl++) {
       const int pw = pl ? w / 2 : w, ph = pl ? h / 2 : h;
-      const int stp = pl ? d->geo.rec_stride_c() : d->geo.rec_stride_y();
+      const int stp = d->lay.stride(pl);
       const uint8_t* from = d->plane0(rec, s, pl) + (size_t)(d->out_cy[i] >> (pl ? 1 : 0)) * stp + (d->out_cx[i] >> (pl ? 1 : 0));
       CK(cudaMemcpy2DAsync(dst, pw, from, stp, pw, ph, cudaMemcpyDeviceToHost, d->st));
       dst += (size_t)pw * ph;
@@ -362,9 +359,8 @@ int b2h264_dec_set_stream(b2h264_dec* d, void* stream) {
   if (!d) return -1;
   CK(cudaSetDevice(d->cfg.device));
   CK(cudaStreamSynchronize(d->st));
-  if (d->own_stream) CK(cudaStreamDestroy(d->st));
+  d->own_st = Stream();
   d->st = (cudaStream_t)stream;
-  d->own_stream = false;
   return 0;
 }
 

@@ -19,6 +19,22 @@ namespace b2h264 {
 // Record: 128-byte head (MbOut bytes [0, 112) + chroma_dc, presence mask of the 24 residual blocks in pad0) + 32 bytes per present block.
 int pack_records_compact(const MbOut* mbs, int n, uint8_t* dst, int32_t* idx);
 
+// A padded picture (picture_handle.cpp:60-85): Y, then Cb, then Cr, luma padded by 32 samples on every side and chroma by 16, so
+// sample (0, 0) lies at row 32, column 32 of the luma plane and at row 16, column 16 of each chroma plane.  Built from the picture
+// size in macroblocks, or from given strides and the height in macroblocks.
+struct PicLayout {
+  int stride_y = 0, stride_c = 0, rows_y = 0, rows_c = 0;
+  PicLayout() = default;
+  PicLayout(int mb_w, int mb_h) : PicLayout(mb_w * 16 + 64, mb_w * 8 + 32, mb_h) {}
+  PicLayout(int sty, int stc, int mb_h) : stride_y(sty), stride_c(stc), rows_y(mb_h * 16 + 64), rows_c(mb_h * 8 + 32) {}
+  int stride(int pl) const { return pl ? stride_c : stride_y; }
+  size_t y_bytes() const { return (size_t)stride_y * rows_y; }
+  size_t c_bytes() const { return (size_t)stride_c * rows_c; }
+  size_t bytes() const { return y_bytes() + 2 * c_bytes(); }
+  // offset of sample (0, 0) of plane pl (0 Y, 1 Cb, 2 Cr) from the first byte of the picture
+  size_t plane0(int pl) const { return pl == 0 ? (size_t)32 * stride_y + 32 : y_bytes() + (size_t)(pl - 1) * c_bytes() + (size_t)16 * stride_c + 16; }
+};
+
 struct StreamCtl {
   StreamParams sp;
   float fps;
@@ -45,11 +61,11 @@ struct StreamCtl {
     sp.dbk_idc = idc == 2 ? 0 : idc; sp.dbk_alpha_div2 = alpha_c0_offset; sp.dbk_beta_div2 = beta_offset;
     return true;
   }
-  // geometry of the padded pictures (picture_handle.cpp:60-85: 32-pixel luma padding)
-  int rec_stride_y() const { return sp.mb_w * 16 + 64; }
-  int rec_stride_c() const { return sp.mb_w * 8 + 32; }
-  int rec_rows_y() const { return sp.mb_h * 16 + 64; }
-  int rec_rows_c() const { return sp.mb_h * 8 + 32; }
+  // geometry of the padded pictures (PicLayout)
+  int rec_stride_y() const { return PicLayout(sp.mb_w, sp.mb_h).stride_y; }
+  int rec_stride_c() const { return PicLayout(sp.mb_w, sp.mb_h).stride_c; }
+  int rec_rows_y() const { return PicLayout(sp.mb_w, sp.mb_h).rows_y; }
+  int rec_rows_c() const { return PicLayout(sp.mb_w, sp.mb_h).rows_c; }
   EncFrameParams frame_params(bool idr, bool ref_is_p) const;
   // serialises the access unit of the frame just coded (SPS+PPS+IDR slice, or P slice)
   void write_access_unit(bool idr, const MbOut* mbs, std::vector<uint8_t>* au);                 // one record per MB

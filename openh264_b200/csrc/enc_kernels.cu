@@ -1196,8 +1196,8 @@ extern "C" int b2h264_debug_decode_records(int n, int mb_w, int mb_h, const int*
   const int n_mb = mb_w * mb_h;
   bool has_b = false;
   for (size_t i = 0; i < (size_t)n * n_mb; i++) has_b = has_b || MBT_IS_B(recs[i].mb_type);
-  const int sty = mb_w * 16 + 64, stc = mb_w * 8 + 32;
-  const size_t y_bytes = (size_t)sty * (mb_h * 16 + 64), c_bytes = (size_t)stc * (mb_h * 8 + 32), pic_bytes = y_bytes + 2 * c_bytes;
+  const b2h264::PicLayout lay(mb_w, mb_h);
+  const size_t pic_bytes = lay.bytes();
   const size_t slots = (size_t)n_refs + 1, dense = (size_t)n_mb * 384;
   uint8_t *d_pic = nullptr, *d_pack = nullptr;
   int32_t* d_idx = nullptr;
@@ -1210,10 +1210,7 @@ extern "C" int b2h264_debug_decode_records(int n, int mb_w, int mb_h, const int*
   std::vector<uint8_t> pack((size_t)n * n_mb * sizeof(MbOut));
   std::vector<int32_t> idx((size_t)n * n_mb);
   std::vector<StreamFrame> h((size_t)n * n_refs);
-  auto plane0 = [&](uint8_t* base, size_t s, size_t slot, int pl) {
-    uint8_t* p = base + (s * slots + slot) * pic_bytes;
-    return pl == 0 ? p + (size_t)32 * sty + 32 : p + y_bytes + (size_t)(pl - 1) * c_bytes + (size_t)16 * stc + 16;
-  };
+  auto plane0 = [&](uint8_t* base, size_t s, size_t slot, int pl) { return base + (s * slots + slot) * pic_bytes + lay.plane0(pl); };
   int rc = (int)cudaMalloc(&d_pic, (size_t)n * slots * pic_bytes + 256);
   if (!rc) rc = (int)cudaMemset(d_pic, 0, (size_t)n * slots * pic_bytes + 256);
   if (!rc) rc = (int)cudaMalloc(&d_pack, pack.size());
@@ -1231,12 +1228,12 @@ extern "C" int b2h264_debug_decode_records(int n, int mb_w, int mb_h, const int*
       const uint8_t* src = refs + (s * n_refs + r) * dense;
       for (int pl = 0; pl < 3 && !rc; pl++) {
         const int w = pl ? 8 * mb_w : 16 * mb_w, hh = pl ? 8 * mb_h : 16 * mb_h;
-        rc = (int)cudaMemcpy2D(plane0(d_pic, s, r, pl), pl ? stc : sty, src + (pl ? (size_t)n_mb * 256 + (size_t)(pl - 1) * n_mb * 64 : 0), w, w, hh,
+        rc = (int)cudaMemcpy2D(plane0(d_pic, s, r, pl), lay.stride(pl), src + (pl ? (size_t)n_mb * 256 + (size_t)(pl - 1) * n_mb * 64 : 0), w, w, hh,
                                cudaMemcpyHostToDevice);
       }
       StreamFrame& F = h[s * n_refs + r];
       memset(&F, 0, sizeof(F));
-      F.p.mb_w = mb_w; F.p.mb_h = mb_h; F.p.rec_stride_y = sty; F.p.rec_stride_c = stc;
+      F.p.mb_w = mb_w; F.p.mb_h = mb_h; F.p.rec_stride_y = lay.stride_y; F.p.rec_stride_c = lay.stride_c;
       for (int pl = 0; pl < 3; pl++) F.f.rec[pl] = plane0(d_pic, s, r, pl);
     }
   if (!rc) rc = (int)cudaMemcpy(d_sf, h.data(), h.size() * sizeof(StreamFrame), cudaMemcpyHostToDevice);
@@ -1255,7 +1252,7 @@ extern "C" int b2h264_debug_decode_records(int n, int mb_w, int mb_h, const int*
   for (int s = 0; s < n && !rc; s++) {
     StreamFrame& F = h[s];
     memset(&F, 0, sizeof(F));
-    F.p.mb_w = mb_w; F.p.mb_h = mb_h; F.p.rec_stride_y = sty; F.p.rec_stride_c = stc;
+    F.p.mb_w = mb_w; F.p.mb_h = mb_h; F.p.rec_stride_y = lay.stride_y; F.p.rec_stride_c = lay.stride_c;
     F.p.mv_range = 64; F.p.dec_mode = 1; F.p.dec_cqp_off = cqp_off[s];
     for (int pl = 0; pl < 3; pl++) { F.f.rec[pl] = plane0(d_pic, s, n_refs, pl); F.f.ref[pl] = F.f.dpb0[pl] = plane0(d_pic, s, 0, pl); }
     F.f.dpb_stride = (int64_t)pic_bytes;

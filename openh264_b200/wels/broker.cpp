@@ -22,40 +22,28 @@ EncPool::EncPool(const PoolKey& key, int capacity, int device) : Batcher(capacit
   cfg.intra_period = key.intra_period;
   cfg.loop_filter_idc = key.dbk_idc; cfg.loop_filter_alpha_c0_offset = key.dbk_alpha; cfg.loop_filter_beta_offset = key.dbk_beta;
   if (b2h264_enc_create(&cfg, &enc_) != 0) { enc_ = nullptr; return; }
-  if (b2h264_enc_set_references(enc_, key.num_ref_frames, key.ltr, 30) != 0) {
+  // on failure ok() is false and the destructor releases what was acquired
+  if (b2h264_enc_set_references(enc_, key.num_ref_frames, key.ltr, 30) != 0 || cudaSetDevice(device) != cudaSuccess ||
+      pinned_.alloc(frame_bytes_ * capacity, cudaHostAllocPortable) != cudaSuccess || d_stage_.alloc(frame_bytes_ * capacity) != cudaSuccess ||
+      up_stream_.create(cudaStreamNonBlocking) != cudaSuccess) {
     b2h264_enc_destroy(enc_);
     enc_ = nullptr;
     return;
   }
-  if (cudaSetDevice(device) != cudaSuccess ||
-      cudaHostAlloc((void**)&pinned_, frame_bytes_ * capacity, cudaHostAllocPortable) != cudaSuccess) {
-    b2h264_enc_destroy(enc_);
-    enc_ = nullptr; pinned_ = nullptr;
-    return;
-  }
-  cudaStream_t us = nullptr;
-  if (cudaMalloc((void**)&d_stage_, frame_bytes_ * capacity) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&us, cudaStreamNonBlocking) != cudaSuccess) {
-    b2h264_enc_destroy(enc_); cudaFreeHost(pinned_); if (d_stage_) cudaFree(d_stage_);
-    enc_ = nullptr; pinned_ = nullptr; d_stage_ = nullptr;
-    return;
-  }
-  up_stream_ = us;
   au_.resize(capacity);
   idr_.assign(capacity, 0);
 }
 
 EncPool::~EncPool() {
+  cudaSetDevice(device_);
+  if (up_stream_.get()) cudaStreamSynchronize(up_stream_.get());
   if (enc_) b2h264_enc_destroy(enc_);
-  if (pinned_) cudaFreeHost(pinned_);
-  if (d_stage_) { cudaSetDevice(device_); cudaFree(d_stage_); }
-  if (up_stream_) cudaStreamDestroy((cudaStream_t)up_stream_);
 }
 
 int EncPool::upload(int slot) {
   if (cudaSetDevice(device_) != cudaSuccess) return -1;
-  return cudaMemcpyAsync(d_stage_ + (size_t)slot * frame_bytes_, pinned_ + (size_t)slot * frame_bytes_, frame_bytes_, cudaMemcpyHostToDevice,
-                         (cudaStream_t)up_stream_) == cudaSuccess ? 0 : -1;
+  return cudaMemcpyAsync(d_stage_.get() + (size_t)slot * frame_bytes_, pinned_.get() + (size_t)slot * frame_bytes_, frame_bytes_, cudaMemcpyHostToDevice,
+                         up_stream_.get()) == cudaSuccess ? 0 : -1;
 }
 
 int EncPool::force_idr(int slot) {
@@ -77,9 +65,9 @@ int EncPool::ltr_mark_period(int slot, int period) {
 void EncPool::code_batch(const std::vector<int>& slots, int* result) {
   std::vector<const uint8_t*> src(cap_, nullptr), bs(cap_, nullptr);
   std::vector<int32_t> nb(cap_, 0), ft(cap_, 0);
-  for (int s : slots) src[s] = d_stage_ + (size_t)s * frame_bytes_;
+  for (int s : slots) src[s] = d_stage_.get() + (size_t)s * frame_bytes_;
   // every stream of the batch enqueued its upload before it joined: one wait covers them all
-  int rc = cudaSetDevice(device_) == cudaSuccess && cudaStreamSynchronize((cudaStream_t)up_stream_) == cudaSuccess ? 0 : -1;
+  int rc = cudaSetDevice(device_) == cudaSuccess && cudaStreamSynchronize(up_stream_.get()) == cudaSuccess ? 0 : -1;
   if (rc == 0) rc = b2h264_enc_submit(enc_, src.data(), 1);
   if (rc == 0) rc = b2h264_enc_collect(enc_, bs.data(), nb.data(), ft.data());
   for (int s : slots) {

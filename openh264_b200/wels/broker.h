@@ -22,6 +22,7 @@
 #include <mutex>
 #include <vector>
 
+#include "../csrc/cuda_owned.h"
 #include "b2h264_codec.h"
 #include "batcher.h"
 
@@ -47,7 +48,7 @@ class EncPool : public Batcher {
   bool ok() const { return enc_ != nullptr; }
   bool serves(const PoolKey& key) const { return key == key_; }
   // the slot's page-locked staging picture: the caller gathers its planes here (tightly packed I420) before upload()
-  uint8_t* staging(int slot) { return pinned_ + (size_t)slot * frame_bytes_; }
+  uint8_t* staging(int slot) { return pinned_.get() + (size_t)slot * frame_bytes_; }
   // starts the host -> device copy of the slot's staged picture right away (on the caller's thread): by the time the last
   // stream of a batch arrives the pictures of the others are already in HBM
   int upload(int slot);
@@ -69,9 +70,9 @@ class EncPool : public Batcher {
   int device_;
   size_t frame_bytes_;
   b2h264_enc* enc_ = nullptr;
-  uint8_t* pinned_ = nullptr;
-  uint8_t* d_stage_ = nullptr;             // device copies of the staged pictures (what the batch reads)
-  void* up_stream_ = nullptr;              // cudaStream_t of the early uploads
+  b2h264::Stream up_stream_;               // the early uploads; released after the buffers below
+  b2h264::HostBuf<uint8_t> pinned_;
+  b2h264::DeviceBuf<uint8_t> d_stage_;     // device copies of the staged pictures (what the batch reads)
   std::vector<std::vector<uint8_t>> au_;
   std::vector<uint8_t> idr_;
 };
