@@ -20,10 +20,13 @@
 #include "enc_frame.cuh"
 #include "dec_mb.cuh"
 #include "dec_records_check.h"
+#include "stage_hooks.cuh"
 #include "enc_launch.h"
 #include "enc_host.h"
+#include "cuda_owned.h"
 
 using namespace mbk;
+using b2h264::DeviceBuf;
 
 namespace mbk {
 __constant__ uint8_t c_alpha[52];
@@ -685,14 +688,14 @@ extern "C" int b2h264_debug_deblock_pictures(int n, uint8_t* const* planes, cons
     h[i].f.mbi = mbi[i];
     h[i].f.dec_aux_b = aux_b ? aux_b[i] : nullptr;
   }
-  StreamFrame* d_sf = nullptr;
-  cudaError_t e = cudaMalloc(&d_sf, sizeof(StreamFrame) * n);
-  if (e != cudaSuccess) return (int)e;
-  rc = (int)cudaMemcpy(d_sf, h.data(), sizeof(StreamFrame) * n, cudaMemcpyHostToDevice);
+  DeviceBuf<StreamFrame> d_sf;
+  rc = (int)d_sf.alloc(sizeof(StreamFrame) * n);
+  if (rc) return rc;
+  rc = (int)cudaMemcpy(d_sf.get(), h.data(), sizeof(StreamFrame) * n, cudaMemcpyHostToDevice);
   int used = 0;
-  if (!rc) rc = bsl ? launch_deblock_t<true>(d_sf, n, max_h, 0, n_warps, &used) : launch_deblock_t<false>(d_sf, n, max_h, 0, n_warps, &used);
+  if (!rc)
+    rc = bsl ? launch_deblock_t<true>(d_sf.get(), n, max_h, 0, n_warps, &used) : launch_deblock_t<false>(d_sf.get(), n, max_h, 0, n_warps, &used);
   if (!rc) rc = (int)cudaDeviceSynchronize();
-  cudaFree(d_sf);
   if (warps_used) *warps_used = used;
   return rc;
 }
@@ -700,48 +703,29 @@ extern "C" int b2h264_debug_deblock_pictures(int n, uint8_t* const* planes, cons
 // arrays: src_pred[768 * i] = case i's source (luma 16x16, Cb 8x8, Cr 8x8, dense) then its prediction in the same layout;
 // qp[i] = its luma QP (the chroma QP follows from the table, as in the encoder); out[kInterResOut * i] = the MbOut record
 // (896 bytes: levels, chroma DC; the rest zero), MbInfo::nnz (24), MbInfo::cbp, 7 zero bytes, the reconstruction (luma 16x16,
-// Cb 8x8, Cr 8x8).  Returns -1 without launching for a bad argument, else the CUDA status.
-constexpr int kInterResOut = (int)sizeof(MbOut) + 32 + 384;
+// Cb 8x8, Cr 8x8).  Returns -1 without launching for a bad argument (stage_hooks.cuh), else the CUDA status.
 __global__ void k_debug_inter_residual(const uint8_t* in, const int* qp, uint8_t* out) {
   extern __shared__ __align__(128) uint8_t smem[];
   MbScratch& s = *reinterpret_cast<MbScratch*>(smem);
-  const int i = blockIdx.x, l = threadIdx.x;
-  for (int w = l; w < (int)(sizeof(MbScratch) / 4); w += 32) reinterpret_cast<uint32_t*>(&s)[w] = 0;
+  const int i = blockIdx.x;
+  for (int w = threadIdx.x; w < (int)(sizeof(MbScratch) / 4); w += 32) reinterpret_cast<uint32_t*>(&s)[w] = 0;
   __syncwarp();
-  const uint8_t* src = in + 768 * i;
-  for (int k = l; k < 256; k += 32) { s.cur_y[k] = src[k]; s.pred_y[0][k] = src[384 + k]; }
-  for (int k = l; k < 128; k += 32) { s.cur_c[k] = src[256 + k]; s.pred_c[0][k] = src[640 + k]; }
-  MbCtx c;
-  memset(&c, 0, sizeof(c));
-  c.qp = qp[i]; c.qp_c = tbl_chroma_qp(c.qp);
-  __syncwarp();
-  inter_residual_pass(c, s, s.pred_y[0], s.pred_c[0]);
-  __syncwarp();
-  uint8_t* o = out + (size_t)kInterResOut * i;
-  for (int k = l; k < (int)sizeof(MbOut); k += 32) o[k] = reinterpret_cast<const uint8_t*>(&s.out)[k];
-  o += sizeof(MbOut);
-  for (int k = l; k < 32; k += 32) o[k] = k < 24 ? (uint8_t)s.info.nnz[k] : k == 24 ? s.info.cbp : 0;
-  o += 32;
-  for (int k = l; k < 384; k += 32)
-    o[k] = k < 256 ? *tile_y(s.tile, k & 15, k >> 4) : *tile_c(k < 320 ? s.tile.u : s.tile.v, k & 7, (k >> 3) & 7);
+  inter_residual_case(in + 768 * i, qp[i], out + (size_t)kInterResOut * i, s);
 }
 extern "C" int b2h264_debug_inter_residual(int n, const uint8_t* src_pred, const int* qp, uint8_t* out) {
-  if (n < 1 || !src_pred || !qp || !out) return -1;
-  for (int i = 0; i < n; i++)
-    if (qp[i] < 0 || qp[i] > 51) return -1;
-  uint8_t *d_in = nullptr, *d_out = nullptr;
-  int* d_qp = nullptr;
-  int rc = (int)cudaMalloc(&d_in, (size_t)768 * n);
-  if (!rc) rc = (int)cudaMalloc(&d_qp, sizeof(int) * n);
-  if (!rc) rc = (int)cudaMalloc(&d_out, (size_t)kInterResOut * n);
-  if (!rc) rc = (int)cudaMemcpy(d_in, src_pred, (size_t)768 * n, cudaMemcpyHostToDevice);
-  if (!rc) rc = (int)cudaMemcpy(d_qp, qp, sizeof(int) * n, cudaMemcpyHostToDevice);
+  if (!inter_residual_args_ok(n, src_pred, qp, out)) return -1;
+  DeviceBuf<uint8_t> d_in, d_out;
+  DeviceBuf<int> d_qp;
+  int rc = (int)d_in.alloc((size_t)768 * n);
+  if (!rc) rc = (int)d_qp.alloc(sizeof(int) * n);
+  if (!rc) rc = (int)d_out.alloc((size_t)kInterResOut * n);
+  if (!rc) rc = (int)cudaMemcpy(d_in.get(), src_pred, (size_t)768 * n, cudaMemcpyHostToDevice);
+  if (!rc) rc = (int)cudaMemcpy(d_qp.get(), qp, sizeof(int) * n, cudaMemcpyHostToDevice);
   if (!rc) {
-    k_debug_inter_residual<<<n, 32, sizeof(MbScratch)>>>(d_in, d_qp, d_out);
+    k_debug_inter_residual<<<n, 32, sizeof(MbScratch)>>>(d_in.get(), d_qp.get(), d_out.get());
     rc = b2h264_launched();
   }
-  if (!rc) rc = (int)cudaMemcpy(out, d_out, (size_t)kInterResOut * n, cudaMemcpyDeviceToHost);
-  cudaFree(d_in); cudaFree(d_qp); cudaFree(d_out);
+  if (!rc) rc = (int)cudaMemcpy(out, d_out.get(), (size_t)kInterResOut * n, cudaMemcpyDeviceToHost);
   return rc;
 }
 // Test hook (not part of the public headers): the intra tail (md_i16x16, then intra_mb_finish, as stage I runs them) on n
@@ -750,65 +734,28 @@ extern "C" int b2h264_debug_inter_residual(int n, const uint8_t* src_pred, const
 // of the I4x4 try (< 0: the I16x16 cost), then int8 I4x4 modes of the left neighbour's right column and of the top
 // neighbour's bottom row (a neighbour whose first entry is < 0 is not I4x4), 8 bytes padding.  out[kIntraTailOut * i] = the
 // MbOut record, the MbInfo record, int32 cost limit used / I4x4 cost returned / lambda / 0, the tile.  Returns -1 without
-// launching for a bad argument, else the CUDA status.
-constexpr int kIntraTailIn = (int)sizeof(RecTile) + 384 + 32;
-constexpr int kIntraTailOut = (int)(sizeof(MbOut) + sizeof(MbInfo)) + 16 + (int)sizeof(RecTile);
+// launching for a bad argument (stage_hooks.cuh), else the CUDA status.
 __global__ void k_debug_intra_tail(const uint8_t* in, int32_t* sad, uint8_t* out) {
   extern __shared__ __align__(128) uint8_t smem[];
   MbScratch& s = *reinterpret_cast<MbScratch*>(smem);
-  const int i = blockIdx.x, l = threadIdx.x;
-  for (int w = l; w < (int)(sizeof(MbScratch) / 4); w += 32) reinterpret_cast<uint32_t*>(&s)[w] = 0;
+  const int i = blockIdx.x;
+  for (int w = threadIdx.x; w < (int)(sizeof(MbScratch) / 4); w += 32) reinterpret_cast<uint32_t*>(&s)[w] = 0;
   __syncwarp();
-  const uint8_t* src = in + (size_t)kIntraTailIn * i;
-  for (int k = l; k < (int)sizeof(RecTile); k += 32) reinterpret_cast<uint8_t*>(&s.tile)[k] = src[k];
-  src += sizeof(RecTile);
-  for (int k = l; k < 256; k += 32) s.cur_y[k] = src[k];
-  for (int k = l; k < 128; k += 32) s.cur_c[k] = src[256 + k];
-  const int32_t* prm = reinterpret_cast<const int32_t*>(src + 384);
-  const int8_t* nm = reinterpret_cast<const int8_t*>(src + 400);
-  if (l == 0)
-    for (int j = 0; j < 8; j++) {
-      MbInfo& m = s.nbi[j < 4 ? 3 : 1];
-      m.mb_type = nm[j & 4] >= 0 ? MBT_I4x4 : MBT_I16x16;
-      m.i4_mode[j < 4 ? 4 * j + 3 : 8 + j] = nm[j];
-    }
-  MbCtx c;
-  memset(&c, 0, sizeof(c));
-  c.qp = prm[0]; c.qp_c = tbl_chroma_qp(c.qp); c.lambda = tbl_lambda(c.qp); c.nb = prm[1];
-  c.p.fast_mode = prm[2]; c.p.mb_w = 1; c.f.sad_cost = sad + i;
-  __syncwarp();
-  int bb;
-  const int cost16 = md_i16x16(c, s, &bb);
-  const int limit = prm[3] < 0 ? cost16 : prm[3];
-  const int cost4 = intra_mb_finish(c, s, limit, bb);
-  __syncwarp();
-  uint8_t* o = out + (size_t)kIntraTailOut * i;
-  for (int k = l; k < (int)sizeof(MbOut); k += 32) o[k] = reinterpret_cast<const uint8_t*>(&s.out)[k];
-  o += sizeof(MbOut);
-  for (int k = l; k < (int)sizeof(MbInfo); k += 32) o[k] = reinterpret_cast<const uint8_t*>(&s.info)[k];
-  o += sizeof(MbInfo);
-  if (l < 4) reinterpret_cast<int32_t*>(o)[l] = l == 0 ? limit : l == 1 ? cost4 : l == 2 ? c.lambda : 0;
-  o += 16;
-  for (int k = l; k < (int)sizeof(RecTile); k += 32) o[k] = reinterpret_cast<const uint8_t*>(&s.tile)[k];
+  intra_tail_case(in + (size_t)kIntraTailIn * i, sad + i, out + (size_t)kIntraTailOut * i, s);
 }
 extern "C" int b2h264_debug_intra_tail(int n, const uint8_t* in, uint8_t* out) {
-  if (n < 1 || !in || !out) return -1;
-  for (int i = 0; i < n; i++) {
-    const int32_t* prm = reinterpret_cast<const int32_t*>(in + (size_t)kIntraTailIn * i + sizeof(RecTile) + 384);
-    if (prm[0] < 0 || prm[0] > 51 || prm[1] < 0 || prm[1] > 15) return -1;
-  }
-  uint8_t *d_in = nullptr, *d_out = nullptr;
-  int32_t* d_sad = nullptr;
-  int rc = (int)cudaMalloc(&d_in, (size_t)kIntraTailIn * n);
-  if (!rc) rc = (int)cudaMalloc(&d_sad, sizeof(int32_t) * n);
-  if (!rc) rc = (int)cudaMalloc(&d_out, (size_t)kIntraTailOut * n);
-  if (!rc) rc = (int)cudaMemcpy(d_in, in, (size_t)kIntraTailIn * n, cudaMemcpyHostToDevice);
+  if (!intra_tail_args_ok(n, in, out)) return -1;
+  DeviceBuf<uint8_t> d_in, d_out;
+  DeviceBuf<int32_t> d_sad;
+  int rc = (int)d_in.alloc((size_t)kIntraTailIn * n);
+  if (!rc) rc = (int)d_sad.alloc(sizeof(int32_t) * n);
+  if (!rc) rc = (int)d_out.alloc((size_t)kIntraTailOut * n);
+  if (!rc) rc = (int)cudaMemcpy(d_in.get(), in, (size_t)kIntraTailIn * n, cudaMemcpyHostToDevice);
   if (!rc) {
-    k_debug_intra_tail<<<n, 32, sizeof(MbScratch)>>>(d_in, d_sad, d_out);
+    k_debug_intra_tail<<<n, 32, sizeof(MbScratch)>>>(d_in.get(), d_sad.get(), d_out.get());
     rc = b2h264_launched();
   }
-  if (!rc) rc = (int)cudaMemcpy(out, d_out, (size_t)kIntraTailOut * n, cudaMemcpyDeviceToHost);
-  cudaFree(d_in); cudaFree(d_sad); cudaFree(d_out);
+  if (!rc) rc = (int)cudaMemcpy(out, d_out.get(), (size_t)kIntraTailOut * n, cudaMemcpyDeviceToHost);
   return rc;
 }
 // Test hook (not part of the public headers): stage B's motion search of one partition shape on n macroblock jobs, one warp
@@ -826,95 +773,33 @@ extern "C" int b2h264_debug_intra_tail(int n, const uint8_t* in, uint8_t* out) {
 // satd_cost, satd, ref - luma sample (0, 0) in bytes), then mv x, y and satd_cost after the refinement, 0; at word 48:
 // win_x0, win_y0, win_ok as issued (win_x0 / win_y0 0 without a window); padding to word 64; then the luma prediction
 // (16 x 16) and the chroma prediction (Cb 8 x 8, Cr 8 x 8).
-// All jobs of a call share stride_y, stride_c and mb_h (one tensor map covers their planes).  Returns -1 without launching for
-// a bad argument (n < 1, QP outside 0..51, a shape or candidate count out of range, a macroblock outside the picture, a luma
-// stride that is not a multiple of 16 or a chroma stride not a multiple of 8, strides narrower than the padded picture, a set
-// larger than set_bytes or set_bytes not a multiple of 16, a negative mv_range: the clip window of the search would no longer
-// keep every block inside the padding), else the CUDA status.
-constexpr int kMeJobIn = 80 * 4 + 256;
-constexpr int kMeJobOut = 64 * 4 + 256 + 128;
+// Returns -1 without launching for a bad argument (stage_hooks.cuh; and see below), else the CUDA status.
 __global__ void k_debug_me_partitions(const uint8_t* planes, long long set_bytes, const uint8_t* jobs, uint8_t* out,
                                       const __grid_constant__ CUtensorMap tm_ref, int has_window) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ WinBar wb;
   MbScratch& s = my_scratch(smem);
-  const int i = blockIdx.x, l = threadIdx.x;
-  for (int w = l; w < (int)(sizeof(MbScratch) / 4); w += 32) reinterpret_cast<uint32_t*>(&s)[w] = 0;
-  if (l == 0) {
+  const int i = blockIdx.x;
+  for (int w = threadIdx.x; w < (int)(sizeof(MbScratch) / 4); w += 32) reinterpret_cast<uint32_t*>(&s)[w] = 0;
+  if (threadIdx.x == 0) {
     wb.phase = 0;
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"((uint32_t)__cvta_generic_to_shared(&wb.bar)));
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  const int32_t* J = reinterpret_cast<const int32_t*>(jobs + (size_t)kMeJobIn * i);
-  for (int k = l; k < 256; k += 32) s.cur_y[k] = jobs[(size_t)kMeJobIn * i + 320 + k];
-  EncFrameParams p;
-  EncFramePtrs f;
-  memset(&p, 0, sizeof(p));
-  memset(&f, 0, sizeof(f));
-  p.mb_w = J[0]; p.mb_h = J[1]; p.rec_stride_y = J[2]; p.rec_stride_c = J[3]; p.mv_range = J[4]; p.qp = J[7]; p.fast_mode = J[8];
-  p.ref_plane = i;
-  const uint8_t* set = planes + (size_t)set_bytes * i;
-  const size_t cb = (size_t)p.rec_stride_y * (16 * p.mb_h + 64), cr = cb + (size_t)p.rec_stride_c * (8 * p.mb_h + 32);
-  f.ref[0] = set + (size_t)32 * p.rec_stride_y + 32;
-  f.ref[1] = set + cb + (size_t)16 * p.rec_stride_c + 16;
-  f.ref[2] = set + cr + (size_t)16 * p.rec_stride_c + 16;
-  mb_ctx(s.ctx, p, f, J[5], J[6]);
-  if (l == 0) { s.ctx.tmap_ref = has_window ? (const void*)&tm_ref : nullptr; s.ctx.wbar = &wb; }
-  __syncwarp();
-  const MbCtx& c = s.ctx;
-  int32_t* o = reinterpret_cast<int32_t*>(out + (size_t)kMeJobOut * i);
-  {
-    int sx, sy;
-    me_start_point(c, J[9], J[10], &sx, &sy);
-    win_issue(c, s, sx, sy);
-    win_wait(c, s);
-  }
-  if (l == 0) { o[48] = s.win_x0; o[49] = s.win_y0; o[50] = s.win_ok; }
-  const int shape = J[11], np = shape == 0 ? 1 : shape == 3 ? 4 : 2;
-  const int blk = shape == 0 ? BLK_16x16 : shape == 1 ? BLK_16x8 : shape == 2 ? BLK_8x16 : BLK_8x8;
-  const int w = shape == 0 || shape == 1 ? 16 : 8, h = shape == 0 || shape == 2 ? 16 : 8;
-  for (int q = 0; q < np; q++) {
-    const int32_t* P = J + 12 + 16 * q;
-    const int ox = shape == 2 ? 8 * q : shape == 3 ? (q & 1) * 8 : 0, oy = shape == 1 ? 8 * q : shape == 3 ? (q >> 1) * 8 : 0;
-    if (l < 10) s.mvcand[l >> 1][l & 1] = (int16_t)P[4 + l];
-    __syncwarp();
-    me_partition(c, s, blk, ox, oy, P[0], P[1], (uint32_t)P[3], P[2], &s.mvcand[0][0], &s.me[q]);
-    const MeState& m = s.me[q];
-    if (l == 0) {
-      int32_t* r = o + 12 * q;
-      r[0] = m.mv_x; r[1] = m.mv_y; r[2] = m.mvp_x; r[3] = m.mvp_y; r[4] = (int32_t)m.sad_cost; r[5] = (int32_t)m.satd_cost;
-      r[6] = m.satd; r[7] = (int32_t)(m.ref - c.f.ref[0]);
-    }
-    __syncwarp();
-  }
-  for (int q = 0; q < np; q++) {
-    const int32_t* P = J + 12 + 16 * q;
-    const int ox = shape == 2 ? 8 * q : shape == 3 ? (q & 1) * 8 : 0, oy = shape == 1 ? 8 * q : shape == 3 ? (q >> 1) * 8 : 0;
-    if (l == 0) { s.me[q].mvp_x = P[14]; s.me[q].mvp_y = P[15]; }
-    __syncwarp();
-    me_refine(c, s, &s.me[q], ox, oy, w, h, s.pred_y[0] + oy * 16 + ox);
-    mc_chroma_part(c, s.pred_c[0], ox, oy, w, h, s.me[q].mv_x, s.me[q].mv_y);
-    if (l == 0) { int32_t* r = o + 12 * q; r[8] = s.me[q].mv_x; r[9] = s.me[q].mv_y; r[10] = (int32_t)s.me[q].satd_cost; }
-    __syncwarp();
-  }
-  uint8_t* ob = out + (size_t)kMeJobOut * i + 256;
-  for (int k = l; k < 256; k += 32) ob[k] = s.pred_y[0][k];
-  for (int k = l; k < 128; k += 32) ob[256 + k] = s.pred_c[0][k];
+  me_partitions_case(i, planes + (size_t)set_bytes * i, jobs + (size_t)kMeJobIn * i, out + (size_t)kMeJobOut * i, s,
+                     has_window ? (const void*)&tm_ref : nullptr, &wb);
 }
 extern "C" int b2h264_debug_me_partitions(int n, const uint8_t* d_planes, long long set_bytes, const uint8_t* jobs, int window,
                                           uint8_t* out) {
-  if (n < 1 || !d_planes || !jobs || !out || set_bytes <= 0 || set_bytes % 16) return -1;
+  if (!me_partitions_args_ok(n, d_planes, set_bytes, jobs, out)) return -1;
+  // Device only: one tensor map covers the planes of every job, so the jobs share stride_y, stride_c and mb_h and the sets
+  // start on 16-byte boundaries; the window copy needs a luma stride that is a multiple of 16 and a chroma one of 8.
   const int32_t* J0 = reinterpret_cast<const int32_t*>(jobs);
+  if (set_bytes % 16) return -1;
   for (int i = 0; i < n; i++) {
     const int32_t* J = reinterpret_cast<const int32_t*>(jobs + (size_t)kMeJobIn * i);
-    const int mb_w = J[0], mb_h = J[1], sy = J[2], sc = J[3];
-    if (mb_w < 1 || mb_h < 1 || sy % 16 || sc % 8 || sy < 16 * mb_w + 64 || sc < 8 * mb_w + 32) return -1;
-    if (sy != J0[2] || sc != J0[3] || mb_h != J0[1]) return -1;
-    if ((long long)sy * (16 * mb_h + 64) + 2LL * sc * (8 * mb_h + 32) > set_bytes) return -1;
-    if (J[4] < 0 || J[5] < 0 || J[5] >= mb_w || J[6] < 0 || J[6] >= mb_h || J[7] < 0 || J[7] > 51 || J[11] < 0 || J[11] > 3) return -1;
-    for (int q = 0; q < 4; q++)
-      if (J[12 + 16 * q + 2] < 0 || J[12 + 16 * q + 2] > 5) return -1;
+    if (J[2] % 16 || J[3] % 8 || J[2] != J0[2] || J[3] != J0[3] || J[1] != J0[1]) return -1;
   }
   alignas(64) CUtensorMap tm;
   memset(&tm, 0, sizeof(tm));
@@ -923,17 +808,15 @@ extern "C" int b2h264_debug_me_partitions(int n, const uint8_t* d_planes, long l
     if (b2h264_make_tmap_planes(&tm, d_planes, (uint64_t)sy, (uint64_t)rows, (uint64_t)n, (uint64_t)sy, (uint64_t)set_bytes, WIN_W, WIN_H))
       return -1;
   }
-  uint8_t *d_jobs = nullptr, *d_out = nullptr;
-  int rc = (int)cudaMalloc(&d_jobs, (size_t)kMeJobIn * n);
-  if (!rc) rc = (int)cudaMalloc(&d_out, (size_t)kMeJobOut * n);
-  if (!rc) rc = (int)cudaMemcpy(d_jobs, jobs, (size_t)kMeJobIn * n, cudaMemcpyHostToDevice);
-  if (!rc) rc = (int)cudaMemset(d_out, 0, (size_t)kMeJobOut * n);
+  DeviceBuf<uint8_t> d_jobs, d_out;
+  int rc = (int)d_jobs.alloc((size_t)kMeJobIn * n);
+  if (!rc) rc = (int)d_out.alloc((size_t)kMeJobOut * n);
+  if (!rc) rc = (int)cudaMemcpy(d_jobs.get(), jobs, (size_t)kMeJobIn * n, cudaMemcpyHostToDevice);
   if (!rc) {
-    k_debug_me_partitions<<<n, 32, sizeof(MbScratch) + 128>>>(d_planes, set_bytes, d_jobs, d_out, tm, window != 0);
+    k_debug_me_partitions<<<n, 32, sizeof(MbScratch) + 128>>>(d_planes, set_bytes, d_jobs.get(), d_out.get(), tm, window != 0);
     rc = b2h264_launched();
   }
-  if (!rc) rc = (int)cudaMemcpy(out, d_out, (size_t)kMeJobOut * n, cudaMemcpyDeviceToHost);
-  cudaFree(d_jobs); cudaFree(d_out);
+  if (!rc) rc = (int)cudaMemcpy(out, d_out.get(), (size_t)kMeJobOut * n, cudaMemcpyDeviceToHost);
   return rc;
 }
 // Test hook (not part of the public headers): stage A's P-skip test on n macroblock jobs, one warp each, in stage A's order:
@@ -947,80 +830,31 @@ extern "C" int b2h264_debug_me_partitions(int n, const uint8_t* d_planes, long l
 // block), SAD cost, skip SAD; padding to word 32; then the current macroblock (Y 16 x 16, Cb 8 x 8, Cr 8 x 8, dense).
 // out[kSkipJobOut * i] (host), int32: ok, skip vector (x, y), the SAD predictor used, cost_luma, cost_skip, the macroblock's
 // sad_cost slot (kSkipSadUnset unless pskip_enc wrote it), 0; then s.skip_pred (384 bytes).
-// Returns -1 without launching for a bad argument (n < 1, QP outside 0..51, a macroblock outside the picture, availability
-// bits or a macroblock type out of range, strides narrower than the padded picture, a set larger than set_bytes), else the
-// CUDA status.
-constexpr int kSkipJobIn = 32 * 4 + 384;
-constexpr int kSkipJobOut = 8 * 4 + 384;
-constexpr int32_t kSkipSadUnset = 0x5a5a5a5a;
+// Returns -1 without launching for a bad argument (stage_hooks.cuh), else the CUDA status.
 __global__ void k_debug_skip_test(const uint8_t* planes, const uint8_t* jobs, int32_t* sad, uint8_t* out) {
   extern __shared__ __align__(128) uint8_t smem[];
   MbScratch& s = my_scratch(smem);
-  const int i = blockIdx.x, l = threadIdx.x;
-  for (int w = l; w < (int)(sizeof(MbScratch) / 4); w += 32) reinterpret_cast<uint32_t*>(&s)[w] = 0;
+  const int i = blockIdx.x;
+  for (int w = threadIdx.x; w < (int)(sizeof(MbScratch) / 4); w += 32) reinterpret_cast<uint32_t*>(&s)[w] = 0;
   __syncwarp();
-  const uint8_t* jb = jobs + (size_t)kSkipJobIn * i;
-  const int32_t* J = reinterpret_cast<const int32_t*>(jb);
-  for (int k = l; k < 256; k += 32) s.cur_y[k] = jb[128 + k];
-  for (int k = l; k < 128; k += 32) s.cur_c[k] = jb[384 + k];
-  if (l < 4) {
-    const int32_t* N = J + 12 + 5 * l;
-    s.nbi[l].mb_type = (uint8_t)N[0];
-    for (int b = 0; b < 16; b++) { s.nbi[l].mv[b][0] = (int16_t)N[1]; s.nbi[l].mv[b][1] = (int16_t)N[2]; }
-    s.nb_sad[l] = N[3];
-    s.nb_skip_sad[l] = N[4];
-  }
-  if (l == 0) { s.col.mb_type = (uint8_t)J[10]; s.col.skip_sad = J[11]; }
-  EncFrameParams p;
-  EncFramePtrs f;
-  memset(&p, 0, sizeof(p));
-  memset(&f, 0, sizeof(f));
-  p.mb_w = J[0]; p.mb_h = J[1]; p.rec_stride_y = J[2]; p.rec_stride_c = J[3]; p.qp = J[6]; p.fast_mode = J[7]; p.ref_is_p = J[9];
-  const size_t cb = (size_t)p.rec_stride_y * (16 * p.mb_h + 64), cr = cb + (size_t)p.rec_stride_c * (8 * p.mb_h + 32);
-  f.ref[0] = planes + (size_t)32 * p.rec_stride_y + 32;
-  f.ref[1] = planes + cb + (size_t)16 * p.rec_stride_c + 16;
-  f.ref[2] = planes + cr + (size_t)16 * p.rec_stride_c + 16;
-  f.sad_cost = sad + i - (J[5] * p.mb_w + J[4]);      // the macroblock's slot is job i's word
-  mb_ctx(s.ctx, p, f, J[4], J[5]);
-  if (l == 0) s.ctx.nb = J[8];
-  __syncwarp();
-  const MbCtx& c = s.ctx;
-  fill_inter_cache(c, s);
-  const int sad_pred = predict_sad_skip(s);
-  const SkipResult r = pskip_enc(c, s, sad_pred);
-  __syncwarp();
-  int32_t* o = reinterpret_cast<int32_t*>(out + (size_t)kSkipJobOut * i);
-  if (l == 0) { o[0] = r.ok; o[1] = r.mvx; o[2] = r.mvy; o[3] = sad_pred; o[4] = r.cost_luma; o[5] = r.cost_skip; o[6] = sad[i]; o[7] = 0; }
-  for (int k = l; k < 384; k += 32) out[(size_t)kSkipJobOut * i + 32 + k] = s.skip_pred[k];
+  skip_test_case(jobs + (size_t)kSkipJobIn * i, planes, sad + i, out + (size_t)kSkipJobOut * i, s);
 }
 extern "C" int b2h264_debug_skip_test(int n, const uint8_t* planes, long long set_bytes, const uint8_t* jobs, uint8_t* out) {
-  if (n < 1 || !planes || !jobs || !out || set_bytes <= 0) return -1;
-  for (int i = 0; i < n; i++) {
-    const int32_t* J = reinterpret_cast<const int32_t*>(jobs + (size_t)kSkipJobIn * i);
-    const int mb_w = J[0], mb_h = J[1], sy = J[2], sc = J[3];
-    if (mb_w < 1 || mb_h < 1 || sy < 16 * mb_w + 64 || sc < 8 * mb_w + 32) return -1;
-    if ((long long)sy * (16 * mb_h + 64) + 2LL * sc * (8 * mb_h + 32) > set_bytes) return -1;
-    if (J[4] < 0 || J[4] >= mb_w || J[5] < 0 || J[5] >= mb_h || J[6] < 0 || J[6] > 51 || J[8] < 0 || J[8] > 15) return -1;
-    if (J[10] < 0 || J[10] > MBT_PSKIP) return -1;
-    for (int k = 0; k < 4; k++)
-      if (J[12 + 5 * k] < 0 || J[12 + 5 * k] > MBT_PSKIP) return -1;
-  }
-  uint8_t *d_planes = nullptr, *d_jobs = nullptr, *d_out = nullptr;
-  int32_t* d_sad = nullptr;
-  int rc = (int)cudaMalloc(&d_planes, (size_t)set_bytes);
-  if (!rc) rc = (int)cudaMalloc(&d_jobs, (size_t)kSkipJobIn * n);
-  if (!rc) rc = (int)cudaMalloc(&d_sad, sizeof(int32_t) * n);
-  if (!rc) rc = (int)cudaMalloc(&d_out, (size_t)kSkipJobOut * n);
-  if (!rc) rc = (int)cudaMemcpy(d_planes, planes, (size_t)set_bytes, cudaMemcpyHostToDevice);
-  if (!rc) rc = (int)cudaMemcpy(d_jobs, jobs, (size_t)kSkipJobIn * n, cudaMemcpyHostToDevice);
-  if (!rc) rc = (int)cudaMemset(d_sad, kSkipSadUnset & 0xff, sizeof(int32_t) * n);
-  if (!rc) rc = (int)cudaMemset(d_out, 0, (size_t)kSkipJobOut * n);
+  if (!skip_test_args_ok(n, planes, set_bytes, jobs, out)) return -1;
+  DeviceBuf<uint8_t> d_planes, d_jobs, d_out;
+  DeviceBuf<int32_t> d_sad;
+  int rc = (int)d_planes.alloc((size_t)set_bytes);
+  if (!rc) rc = (int)d_jobs.alloc((size_t)kSkipJobIn * n);
+  if (!rc) rc = (int)d_sad.alloc(sizeof(int32_t) * n);
+  if (!rc) rc = (int)d_out.alloc((size_t)kSkipJobOut * n);
+  if (!rc) rc = (int)cudaMemcpy(d_planes.get(), planes, (size_t)set_bytes, cudaMemcpyHostToDevice);
+  if (!rc) rc = (int)cudaMemcpy(d_jobs.get(), jobs, (size_t)kSkipJobIn * n, cudaMemcpyHostToDevice);
+  if (!rc) rc = (int)cudaMemset(d_sad.get(), kSkipSadUnset & 0xff, sizeof(int32_t) * n);
   if (!rc) {
-    k_debug_skip_test<<<n, 32, sizeof(MbScratch) + 128>>>(d_planes, d_jobs, d_sad, d_out);
+    k_debug_skip_test<<<n, 32, sizeof(MbScratch) + 128>>>(d_planes.get(), d_jobs.get(), d_sad.get(), d_out.get());
     rc = b2h264_launched();
   }
-  if (!rc) rc = (int)cudaMemcpy(out, d_out, (size_t)kSkipJobOut * n, cudaMemcpyDeviceToHost);
-  cudaFree(d_planes); cudaFree(d_jobs); cudaFree(d_sad); cudaFree(d_out);
+  if (!rc) rc = (int)cudaMemcpy(out, d_out.get(), (size_t)kSkipJobOut * n, cudaMemcpyDeviceToHost);
   return rc;
 }
 static int launch_deblock(const StreamFrame* d_sf, int n_streams, int mb_h, cudaStream_t st, bool b_slices = false) {
@@ -1199,73 +1033,72 @@ extern "C" int b2h264_debug_decode_records(int n, int mb_w, int mb_h, const int*
   const b2h264::PicLayout lay(mb_w, mb_h);
   const size_t pic_bytes = lay.bytes();
   const size_t slots = (size_t)n_refs + 1, dense = (size_t)n_mb * 384;
-  uint8_t *d_pic = nullptr, *d_pack = nullptr;
-  int32_t* d_idx = nullptr;
-  int* d_ws = nullptr;
-  MbOut* d_recs = nullptr;
-  DecMbAux* d_aux = nullptr;
-  DecMbAuxB* d_aux_b = nullptr;
-  MbInfo* d_mbi = nullptr;
-  StreamFrame* d_sf = nullptr;
+  DeviceBuf<uint8_t> d_pic, d_pack;
+  DeviceBuf<int32_t> d_idx;
+  DeviceBuf<int> d_ws;
+  DeviceBuf<MbOut> d_recs;
+  DeviceBuf<DecMbAux> d_aux;
+  DeviceBuf<DecMbAuxB> d_aux_b;
+  DeviceBuf<MbInfo> d_mbi;
+  DeviceBuf<StreamFrame> d_sf;
   std::vector<uint8_t> pack((size_t)n * n_mb * sizeof(MbOut));
   std::vector<int32_t> idx((size_t)n * n_mb);
   std::vector<StreamFrame> h((size_t)n * n_refs);
   auto plane0 = [&](uint8_t* base, size_t s, size_t slot, int pl) { return base + (s * slots + slot) * pic_bytes + lay.plane0(pl); };
-  int rc = (int)cudaMalloc(&d_pic, (size_t)n * slots * pic_bytes + 256);
-  if (!rc) rc = (int)cudaMemset(d_pic, 0, (size_t)n * slots * pic_bytes + 256);
-  if (!rc) rc = (int)cudaMalloc(&d_pack, pack.size());
-  if (!rc) rc = (int)cudaMalloc(&d_idx, idx.size() * sizeof(int32_t));
-  if (!rc) rc = (int)cudaMalloc(&d_recs, (size_t)n * n_mb * sizeof(MbOut));
-  if (!rc) rc = (int)cudaMalloc(&d_aux, (size_t)n * n_mb * sizeof(DecMbAux));
-  if (!rc && has_b) rc = (int)cudaMalloc(&d_aux_b, (size_t)n * n_mb * sizeof(DecMbAuxB));
-  if (!rc) rc = (int)cudaMalloc(&d_mbi, (size_t)n * n_mb * sizeof(MbInfo));
-  if (!rc) rc = (int)cudaMemset(d_mbi, 0, (size_t)n * n_mb * sizeof(MbInfo));
-  if (!rc) rc = (int)cudaMalloc(&d_sf, h.size() * sizeof(StreamFrame));
-  if (!rc) rc = (int)cudaMalloc(&d_ws, dec_sched_ints(n, mb_w, mb_h) * sizeof(int));
+  int rc = (int)d_pic.alloc((size_t)n * slots * pic_bytes + 256);
+  if (!rc) rc = (int)cudaMemset(d_pic.get(), 0, (size_t)n * slots * pic_bytes + 256);
+  if (!rc) rc = (int)d_pack.alloc(pack.size());
+  if (!rc) rc = (int)d_idx.alloc(idx.size() * sizeof(int32_t));
+  if (!rc) rc = (int)d_recs.alloc((size_t)n * n_mb * sizeof(MbOut));
+  if (!rc) rc = (int)d_aux.alloc((size_t)n * n_mb * sizeof(DecMbAux));
+  if (!rc && has_b) rc = (int)d_aux_b.alloc((size_t)n * n_mb * sizeof(DecMbAuxB));
+  if (!rc) rc = (int)d_mbi.alloc((size_t)n * n_mb * sizeof(MbInfo));
+  if (!rc) rc = (int)cudaMemset(d_mbi.get(), 0, (size_t)n * n_mb * sizeof(MbInfo));
+  if (!rc) rc = (int)d_sf.alloc(h.size() * sizeof(StreamFrame));
+  if (!rc) rc = (int)d_ws.alloc(dec_sched_ints(n, mb_w, mb_h) * sizeof(int));
   // the reference pictures into their slots, then their borders as the decoder replicates them after decoding a picture
   for (size_t s = 0; s < (size_t)n && !rc; s++)
     for (size_t r = 0; r < (size_t)n_refs && !rc; r++) {
       const uint8_t* src = refs + (s * n_refs + r) * dense;
       for (int pl = 0; pl < 3 && !rc; pl++) {
         const int w = pl ? 8 * mb_w : 16 * mb_w, hh = pl ? 8 * mb_h : 16 * mb_h;
-        rc = (int)cudaMemcpy2D(plane0(d_pic, s, r, pl), lay.stride(pl), src + (pl ? (size_t)n_mb * 256 + (size_t)(pl - 1) * n_mb * 64 : 0), w, w, hh,
+        rc = (int)cudaMemcpy2D(plane0(d_pic.get(), s, r, pl), lay.stride(pl), src + (pl ? (size_t)n_mb * 256 + (size_t)(pl - 1) * n_mb * 64 : 0), w, w, hh,
                                cudaMemcpyHostToDevice);
       }
       StreamFrame& F = h[s * n_refs + r];
       memset(&F, 0, sizeof(F));
       F.p.mb_w = mb_w; F.p.mb_h = mb_h; F.p.rec_stride_y = lay.stride_y; F.p.rec_stride_c = lay.stride_c;
-      for (int pl = 0; pl < 3; pl++) F.f.rec[pl] = plane0(d_pic, s, r, pl);
+      for (int pl = 0; pl < 3; pl++) F.f.rec[pl] = plane0(d_pic.get(), s, r, pl);
     }
-  if (!rc) rc = (int)cudaMemcpy(d_sf, h.data(), h.size() * sizeof(StreamFrame), cudaMemcpyHostToDevice);
-  if (!rc) rc = launch_expand(d_sf, n * n_refs, mb_w, mb_h, 0);
+  if (!rc) rc = (int)cudaMemcpy(d_sf.get(), h.data(), h.size() * sizeof(StreamFrame), cudaMemcpyHostToDevice);
+  if (!rc) rc = launch_expand(d_sf.get(), n * n_refs, mb_w, mb_h, 0);
   if (!rc) rc = (int)cudaDeviceSynchronize();
   // the records: compact form per stream, unpacked on the device as b2h264_dec_decode does it
   for (int s = 0; s < n && !rc; s++) {
     const int units = b2h264::pack_records_compact(recs + (size_t)s * n_mb, n_mb, pack.data() + (size_t)s * n_mb * sizeof(MbOut), idx.data() + (size_t)s * n_mb);
     if (units > 0)
-      rc = (int)cudaMemcpy(d_pack + (size_t)s * n_mb * sizeof(MbOut), pack.data() + (size_t)s * n_mb * sizeof(MbOut), (size_t)units * 32, cudaMemcpyHostToDevice);
+      rc = (int)cudaMemcpy(d_pack.get() + (size_t)s * n_mb * sizeof(MbOut), pack.data() + (size_t)s * n_mb * sizeof(MbOut), (size_t)units * 32, cudaMemcpyHostToDevice);
   }
-  if (!rc) rc = (int)cudaMemcpy(d_idx, idx.data(), idx.size() * sizeof(int32_t), cudaMemcpyHostToDevice);
-  if (!rc) rc = dec_launch_unpack(d_pack, (size_t)n_mb * sizeof(MbOut), d_idx, d_recs, n, n_mb, 0);
-  if (!rc) rc = (int)cudaMemcpy(d_aux, aux, (size_t)n * n_mb * sizeof(DecMbAux), cudaMemcpyHostToDevice);
-  if (!rc && has_b) rc = (int)cudaMemcpy(d_aux_b, aux_b, (size_t)n * n_mb * sizeof(DecMbAuxB), cudaMemcpyHostToDevice);
+  if (!rc) rc = (int)cudaMemcpy(d_idx.get(), idx.data(), idx.size() * sizeof(int32_t), cudaMemcpyHostToDevice);
+  if (!rc) rc = dec_launch_unpack(d_pack.get(), (size_t)n_mb * sizeof(MbOut), d_idx.get(), d_recs.get(), n, n_mb, 0);
+  if (!rc) rc = (int)cudaMemcpy(d_aux.get(), aux, (size_t)n * n_mb * sizeof(DecMbAux), cudaMemcpyHostToDevice);
+  if (!rc && has_b) rc = (int)cudaMemcpy(d_aux_b.get(), aux_b, (size_t)n * n_mb * sizeof(DecMbAuxB), cudaMemcpyHostToDevice);
   for (int s = 0; s < n && !rc; s++) {
     StreamFrame& F = h[s];
     memset(&F, 0, sizeof(F));
     F.p.mb_w = mb_w; F.p.mb_h = mb_h; F.p.rec_stride_y = lay.stride_y; F.p.rec_stride_c = lay.stride_c;
     F.p.mv_range = 64; F.p.dec_mode = 1; F.p.dec_cqp_off = cqp_off[s];
-    for (int pl = 0; pl < 3; pl++) { F.f.rec[pl] = plane0(d_pic, s, n_refs, pl); F.f.ref[pl] = F.f.dpb0[pl] = plane0(d_pic, s, 0, pl); }
+    for (int pl = 0; pl < 3; pl++) { F.f.rec[pl] = plane0(d_pic.get(), s, n_refs, pl); F.f.ref[pl] = F.f.dpb0[pl] = plane0(d_pic.get(), s, 0, pl); }
     F.f.dpb_stride = (int64_t)pic_bytes;
-    F.f.mbi = d_mbi + (size_t)s * n_mb;
-    F.f.dec_aux_b = has_b ? d_aux_b + (size_t)s * n_mb : nullptr;
+    F.f.mbi = d_mbi.get() + (size_t)s * n_mb;
+    F.f.dec_aux_b = has_b ? d_aux_b.get() + (size_t)s * n_mb : nullptr;
   }
-  if (!rc) rc = (int)cudaMemcpy(d_sf, h.data(), (size_t)n * sizeof(StreamFrame), cudaMemcpyHostToDevice);
-  if (!rc) rc = dec_launch_frame(d_sf, n, mb_w, mb_h, d_ws, d_recs, d_aux, 0, 0, has_b ? 1 : 0);
+  if (!rc) rc = (int)cudaMemcpy(d_sf.get(), h.data(), (size_t)n * sizeof(StreamFrame), cudaMemcpyHostToDevice);
+  if (!rc) rc = dec_launch_frame(d_sf.get(), n, mb_w, mb_h, d_ws.get(), d_recs.get(), d_aux.get(), 0, 0, has_b ? 1 : 0);
   if (!rc) rc = (int)cudaDeviceSynchronize();
   for (int s = 0; s < n && !rc; s++)
-    rc = (int)cudaMemcpy(planes + (size_t)s * pic_bytes, d_pic + ((size_t)s * slots + n_refs) * pic_bytes, pic_bytes, cudaMemcpyDeviceToHost);
-  if (!rc) rc = (int)cudaMemcpy(mbi, d_mbi, (size_t)n * n_mb * sizeof(MbInfo), cudaMemcpyDeviceToHost);
-  cudaFree(d_pic); cudaFree(d_pack); cudaFree(d_idx); cudaFree(d_recs); cudaFree(d_aux); cudaFree(d_aux_b); cudaFree(d_mbi); cudaFree(d_sf); cudaFree(d_ws);
+    rc = (int)cudaMemcpy(planes + (size_t)s * pic_bytes, d_pic.get() + ((size_t)s * slots + n_refs) * pic_bytes, pic_bytes, cudaMemcpyDeviceToHost);
+  if (!rc) rc = (int)cudaMemcpy(mbi, d_mbi.get(), (size_t)n * n_mb * sizeof(MbInfo), cudaMemcpyDeviceToHost);
   return rc;
 }
 

@@ -10,7 +10,6 @@ records only for B macroblocks.  Samples are smooth blocks with steps mostly bel
 so that every filter branch runs.
 """
 import ctypes as C
-import os
 
 import numpy as np
 
@@ -254,29 +253,13 @@ def oracle_deblock(p, stats=None):
     return out
 
 
-_emu = None
-
-
-def emu():
-    """tests/emu/libb2h264_emu.so (host build of the device code), built on first use"""
-    global _emu
-    if _emu is None:
-        import subprocess
-        subprocess.check_call(["make", "-s", "-C", os.path.join(h264lib.ROOT, "tests", "emu")])
-        E = C.CDLL(os.path.join(h264lib.ROOT, "tests", "emu", "libb2h264_emu.so"))
-        E.emu_deblock_picture.restype = C.c_int
-        E.emu_deblock_picture.argtypes = [C.c_void_p] * 3 + [C.c_int] * 4 + [C.c_void_p, C.c_void_p] + [C.c_int] * 4
-        _emu = E
-    return _emu
-
-
 def emu_deblock(p):
     """the picture's planes after the host build of the device filter (deblock_frame_host)"""
     out = [a.copy() for a in p.planes]
     mbi = p.mbi.copy()
     auxb = None if p.auxb is None else p.auxb.copy()
     sy, sc = strides(p.mb_w)
-    rc = emu().emu_deblock_picture(*[out[pl].ctypes.data + p.origin(pl) for pl in range(3)], sy, sc, p.mb_w, p.mb_h,
+    rc = h264lib.emu().emu_deblock_picture(*[out[pl].ctypes.data + p.origin(pl) for pl in range(3)], sy, sc, p.mb_w, p.mb_h,
                                    mbi.ctypes.data, None if auxb is None else auxb.ctypes.data, p.dec_mode, *p.enc_ctl)
     assert rc == 0
     return out

@@ -11,6 +11,7 @@
 #include "../../openh264_b200/csrc/enc_frame.cuh"
 #include "../../openh264_b200/csrc/dec_mb.cuh"
 #include "../../openh264_b200/csrc/dec_records_check.h"
+#include "../../openh264_b200/csrc/enc_host.h"
 
 using namespace mbk;
 
@@ -22,29 +23,26 @@ extern "C" int emu_decode_records(int n, int mb_w, int mb_h, const int* cqp_off,
   if (!dec_records_ok(n, mb_w, mb_h, cqp_off, recs, aux, aux_b, n_refs, refs, planes, mbi)) return -1;
   const int n_mb = mb_w * mb_h;
   b2h264_build_host_tables();
-  const int sty = mb_w * 16 + 64, stc = mb_w * 8 + 32;
-  const size_t y_bytes = (size_t)sty * (mb_h * 16 + 64), c_bytes = (size_t)stc * (mb_h * 8 + 32), pic_bytes = y_bytes + 2 * c_bytes;
+  const b2h264::PicLayout lay(mb_w, mb_h);
+  const size_t pic_bytes = lay.bytes();
   const size_t dense = (size_t)n_mb * 384;
   std::vector<uint8_t> dpb(((size_t)n_refs + 1) * pic_bytes + 256);
   static MbScratch scratch;
   for (int s = 0; s < n; s++) {
     EncFrameParams p;
     memset(&p, 0, sizeof(p));
-    p.mb_w = mb_w; p.mb_h = mb_h; p.rec_stride_y = sty; p.rec_stride_c = stc;
+    p.mb_w = mb_w; p.mb_h = mb_h; p.rec_stride_y = lay.stride_y; p.rec_stride_c = lay.stride_c;
     p.mv_range = 64; p.dec_mode = 1; p.dec_cqp_off = cqp_off[s];
     EncFramePtrs f;
     memset(&f, 0, sizeof(f));
     std::fill(dpb.begin(), dpb.end(), 0);
-    auto plane0 = [&](int slot, int pl) {
-      uint8_t* q = dpb.data() + (size_t)slot * pic_bytes;
-      return pl == 0 ? q + (size_t)32 * sty + 32 : q + y_bytes + (size_t)(pl - 1) * c_bytes + (size_t)16 * stc + 16;
-    };
+    auto plane0 = [&](int slot, int pl) { return dpb.data() + (size_t)slot * pic_bytes + lay.plane0(pl); };
     for (int r = 0; r < n_refs; r++) {
       const uint8_t* src = refs + ((size_t)s * n_refs + r) * dense;
       for (int pl = 0; pl < 3; pl++) {
         const int w = pl ? 8 * mb_w : 16 * mb_w, h = pl ? 8 * mb_h : 16 * mb_h;
         const uint8_t* from = src + (pl ? (size_t)n_mb * 256 + (size_t)(pl - 1) * n_mb * 64 : 0);
-        for (int y = 0; y < h; y++) memcpy(plane0(r, pl) + (size_t)y * (pl ? stc : sty), from + (size_t)y * w, w);
+        for (int y = 0; y < h; y++) memcpy(plane0(r, pl) + (size_t)y * lay.stride(pl), from + (size_t)y * w, w);
         f.rec[pl] = plane0(r, pl);
       }
       emu_expand_frame(p, f);

@@ -1,40 +1,22 @@
 // tests/emu/inter_residual_hooks.cu — test hooks of stage B's residual step for the host emulation build (TEST INFRASTRUCTURE
-// ONLY).  Linked with emu.cu into the library tests/test_gpu_inter_residual.py builds.  emu_inter_residual runs the host build
-// of inter_residual_pass (the serial reference sequence) with the layout of the device hook b2h264_debug_inter_residual
-// (enc_kernels.cu); the outcome counters (enc_inter.cuh: g_res_outcome) are filled by every emu_encode.
+// ONLY).  emu_inter_residual is the host build of the device hook b2h264_debug_inter_residual (enc_kernels.cu), same layout
+// and refusals; the outcome counters (enc_inter.cuh: g_res_outcome) are filled by every emu_encode.
 #include <stdint.h>
 #include <string.h>
 
-#include "../../openh264_b200/csrc/enc_frame.cuh"
+#include "../../openh264_b200/csrc/stage_hooks.cuh"
 
 using namespace mbk;
 
 extern "C" void b2h264_build_host_tables();
 
 extern "C" int emu_inter_residual(int n, const uint8_t* src_pred, const int* qp, uint8_t* out) {
-  if (n < 1 || !src_pred || !qp || !out) return -1;
+  if (!inter_residual_args_ok(n, src_pred, qp, out)) return -1;
   b2h264_build_host_tables();
   static MbScratch s;
-  const int out_bytes = (int)sizeof(MbOut) + 32 + 384;
   for (int i = 0; i < n; i++) {
-    if (qp[i] < 0 || qp[i] > 51) return -1;
     memset(&s, 0, sizeof(s));
-    const uint8_t* src = src_pred + 768 * i;
-    memcpy(s.cur_y, src, 256); memcpy(s.cur_c, src + 256, 128);
-    memcpy(s.pred_y[0], src + 384, 256); memcpy(s.pred_c[0], src + 640, 128);
-    MbCtx c;
-    memset(&c, 0, sizeof(c));
-    c.qp = qp[i]; c.qp_c = tbl_chroma_qp(c.qp);
-    inter_residual_pass(c, s, s.pred_y[0], s.pred_c[0]);
-    uint8_t* o = out + (size_t)out_bytes * i;
-    memcpy(o, &s.out, sizeof(MbOut));
-    o += sizeof(MbOut);
-    memset(o, 0, 32);
-    memcpy(o, s.info.nnz, 24);
-    o[24] = s.info.cbp;
-    o += 32;
-    for (int k = 0; k < 384; k++)
-      o[k] = k < 256 ? *tile_y(s.tile, k & 15, k >> 4) : *tile_c(k < 320 ? s.tile.u : s.tile.v, k & 7, (k >> 3) & 7);
+    inter_residual_case(src_pred + 768 * i, qp[i], out + (size_t)kInterResOut * i, s);
   }
   return 0;
 }

@@ -1,54 +1,23 @@
-// tests/emu/intra_tail_hooks.cu — test hooks of the intra tail for the host emulation build (TEST INFRASTRUCTURE ONLY).  Linked
-// with emu.cu into the library tests/test_gpu_intra_tail.py builds.  emu_intra_tail runs the host build of md_i16x16 +
-// intra_mb_finish (the serial reference sequence) with the layout of the device hook b2h264_debug_intra_tail (enc_kernels.cu);
-// the I4x4 outcome counters (enc_mb.cuh: g_i4_end) are filled by every intra tail the host build runs.
+// tests/emu/intra_tail_hooks.cu — test hooks of the intra tail for the host emulation build (TEST INFRASTRUCTURE ONLY).
+// emu_intra_tail is the host build of the device hook b2h264_debug_intra_tail (enc_kernels.cu), same layout and refusals; the
+// I4x4 outcome counters (enc_mb.cuh: g_i4_end) are filled by every intra tail the host build runs.
 #include <stdint.h>
 #include <string.h>
 
-#include "../../openh264_b200/csrc/enc_frame.cuh"
+#include "../../openh264_b200/csrc/stage_hooks.cuh"
 
 using namespace mbk;
 
 extern "C" void b2h264_build_host_tables();
 
 extern "C" int emu_intra_tail(int n, const uint8_t* in, uint8_t* out) {
-  if (n < 1 || !in || !out) return -1;
+  if (!intra_tail_args_ok(n, in, out)) return -1;
   b2h264_build_host_tables();
   static MbScratch s;
-  const int in_bytes = (int)sizeof(RecTile) + 384 + 32;
-  const int out_bytes = (int)(sizeof(MbOut) + sizeof(MbInfo)) + 16 + (int)sizeof(RecTile);
   for (int i = 0; i < n; i++) {
-    const uint8_t* src = in + (size_t)in_bytes * i;
-    const int32_t* prm = reinterpret_cast<const int32_t*>(src + sizeof(RecTile) + 384);
-    const int8_t* nm = reinterpret_cast<const int8_t*>(src + sizeof(RecTile) + 400);
-    if (prm[0] < 0 || prm[0] > 51 || prm[1] < 0 || prm[1] > 15) return -1;
     memset(&s, 0, sizeof(s));
-    memcpy(&s.tile, src, sizeof(RecTile));
-    memcpy(s.cur_y, src + sizeof(RecTile), 256);
-    memcpy(s.cur_c, src + sizeof(RecTile) + 256, 128);
-    for (int j = 0; j < 8; j++) {
-      MbInfo& m = s.nbi[j < 4 ? 3 : 1];
-      m.mb_type = nm[j & 4] >= 0 ? MBT_I4x4 : MBT_I16x16;
-      m.i4_mode[j < 4 ? 4 * j + 3 : 8 + j] = nm[j];
-    }
     int32_t sad = 0;
-    MbCtx c;
-    memset(&c, 0, sizeof(c));
-    c.qp = prm[0]; c.qp_c = tbl_chroma_qp(c.qp); c.lambda = tbl_lambda(c.qp); c.nb = prm[1];
-    c.p.fast_mode = prm[2]; c.p.mb_w = 1; c.f.sad_cost = &sad;
-    int bb;
-    const int cost16 = md_i16x16(c, s, &bb);
-    const int limit = prm[3] < 0 ? cost16 : prm[3];
-    const int cost4 = intra_mb_finish(c, s, limit, bb);
-    uint8_t* o = out + (size_t)out_bytes * i;
-    memcpy(o, &s.out, sizeof(MbOut));
-    o += sizeof(MbOut);
-    memcpy(o, &s.info, sizeof(MbInfo));
-    o += sizeof(MbInfo);
-    const int32_t tail[4] = {limit, cost4, c.lambda, 0};
-    memcpy(o, tail, 16);
-    o += 16;
-    memcpy(o, &s.tile, sizeof(RecTile));
+    intra_tail_case(in + (size_t)kIntraTailIn * i, &sad, out + (size_t)kIntraTailOut * i, s);
   }
   return 0;
 }

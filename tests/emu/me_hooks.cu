@@ -1,12 +1,11 @@
-// tests/emu/me_hooks.cu — test hooks of stage B's motion search for the host emulation build (TEST INFRASTRUCTURE ONLY).
-// Linked with emu.cu into the library tests/test_gpu_motion_search.py builds.  emu_me_partitions runs the host build of stage
-// B's search sequence (me_start_point, win_issue / win_wait, me_partition per partition, me_refine and mc_chroma_part per
-// partition) with the job and output layout of the device hook b2h264_debug_me_partitions (enc_kernels.cu).  The host build
-// has no search window (win_issue leaves win_ok 0): every search and refinement reads the planes.
+// tests/emu/me_hooks.cu — test hook of stage B's motion search for the host emulation build (TEST INFRASTRUCTURE ONLY).
+// emu_me_partitions is the host build of the device hook b2h264_debug_me_partitions (enc_kernels.cu), with its layout and the
+// refusals both builds share.  The host build has no search window (win_issue leaves win_ok 0): every search and refinement
+// reads the planes.
 #include <stdint.h>
 #include <string.h>
 
-#include "../../openh264_b200/csrc/enc_frame.cuh"
+#include "../../openh264_b200/csrc/stage_hooks.cuh"
 
 using namespace mbk;
 
@@ -14,63 +13,12 @@ extern "C" void b2h264_build_host_tables();
 
 // planes: HOST memory, job i's set at planes + i * set_bytes (layout as the device hook)
 extern "C" int emu_me_partitions(int n, const uint8_t* planes, long long set_bytes, const uint8_t* jobs, uint8_t* out) {
-  const int in_bytes = 80 * 4 + 256, out_bytes = 64 * 4 + 256 + 128;
-  if (n < 1 || !planes || !jobs || !out || set_bytes <= 0) return -1;
+  if (!me_partitions_args_ok(n, planes, set_bytes, jobs, out)) return -1;
   b2h264_build_host_tables();
   static MbScratch s;
   for (int i = 0; i < n; i++) {
-    const int32_t* J = reinterpret_cast<const int32_t*>(jobs + (size_t)in_bytes * i);
-    if (J[7] < 0 || J[7] > 51 || J[11] < 0 || J[11] > 3 || J[5] < 0 || J[5] >= J[0] || J[6] < 0 || J[6] >= J[1] || J[4] < 0) return -1;
     memset(&s, 0, sizeof(s));
-    memcpy(s.cur_y, jobs + (size_t)in_bytes * i + 320, 256);
-    EncFrameParams p;
-    EncFramePtrs f;
-    memset(&p, 0, sizeof(p));
-    memset(&f, 0, sizeof(f));
-    p.mb_w = J[0]; p.mb_h = J[1]; p.rec_stride_y = J[2]; p.rec_stride_c = J[3]; p.mv_range = J[4]; p.qp = J[7]; p.fast_mode = J[8];
-    p.ref_plane = i;
-    const uint8_t* set = planes + (size_t)set_bytes * i;
-    const size_t cb = (size_t)p.rec_stride_y * (16 * p.mb_h + 64), cr = cb + (size_t)p.rec_stride_c * (8 * p.mb_h + 32);
-    f.ref[0] = set + (size_t)32 * p.rec_stride_y + 32;
-    f.ref[1] = set + cb + (size_t)16 * p.rec_stride_c + 16;
-    f.ref[2] = set + cr + (size_t)16 * p.rec_stride_c + 16;
-    mb_ctx(s.ctx, p, f, J[5], J[6]);
-    const MbCtx& c = s.ctx;
-    int32_t* o = reinterpret_cast<int32_t*>(out + (size_t)out_bytes * i);
-    memset(o, 0, out_bytes);
-    {
-      int sx, sy;
-      me_start_point(c, J[9], J[10], &sx, &sy);
-      win_issue(c, s, sx, sy);
-      win_wait(c, s);
-    }
-    o[48] = s.win_x0; o[49] = s.win_y0; o[50] = s.win_ok;
-    const int shape = J[11], np = shape == 0 ? 1 : shape == 3 ? 4 : 2;
-    const int blk = shape == 0 ? BLK_16x16 : shape == 1 ? BLK_16x8 : shape == 2 ? BLK_8x16 : BLK_8x8;
-    const int w = shape == 0 || shape == 1 ? 16 : 8, h = shape == 0 || shape == 2 ? 16 : 8;
-    for (int q = 0; q < np; q++) {
-      const int32_t* P = J + 12 + 16 * q;
-      const int ox = shape == 2 ? 8 * q : shape == 3 ? (q & 1) * 8 : 0, oy = shape == 1 ? 8 * q : shape == 3 ? (q >> 1) * 8 : 0;
-      if (P[2] < 0 || P[2] > 5) return -1;
-      for (int k = 0; k < 10; k++) s.mvcand[k >> 1][k & 1] = (int16_t)P[4 + k];
-      me_partition(c, s, blk, ox, oy, P[0], P[1], (uint32_t)P[3], P[2], &s.mvcand[0][0], &s.me[q]);
-      const MeState& m = s.me[q];
-      int32_t* r = o + 12 * q;
-      r[0] = m.mv_x; r[1] = m.mv_y; r[2] = m.mvp_x; r[3] = m.mvp_y; r[4] = (int32_t)m.sad_cost; r[5] = (int32_t)m.satd_cost;
-      r[6] = m.satd; r[7] = (int32_t)(m.ref - c.f.ref[0]);
-    }
-    for (int q = 0; q < np; q++) {
-      const int32_t* P = J + 12 + 16 * q;
-      const int ox = shape == 2 ? 8 * q : shape == 3 ? (q & 1) * 8 : 0, oy = shape == 1 ? 8 * q : shape == 3 ? (q >> 1) * 8 : 0;
-      s.me[q].mvp_x = P[14]; s.me[q].mvp_y = P[15];
-      me_refine(c, s, &s.me[q], ox, oy, w, h, s.pred_y[0] + oy * 16 + ox);
-      mc_chroma_part(c, s.pred_c[0], ox, oy, w, h, s.me[q].mv_x, s.me[q].mv_y);
-      int32_t* r = o + 12 * q;
-      r[8] = s.me[q].mv_x; r[9] = s.me[q].mv_y; r[10] = (int32_t)s.me[q].satd_cost;
-    }
-    uint8_t* ob = out + (size_t)out_bytes * i + 256;
-    memcpy(ob, s.pred_y[0], 256);
-    memcpy(ob + 256, s.pred_c[0], 128);
+    me_partitions_case(i, planes + (size_t)set_bytes * i, jobs + (size_t)kMeJobIn * i, out + (size_t)kMeJobOut * i, s, nullptr, nullptr);
   }
   return 0;
 }

@@ -1,11 +1,10 @@
-// tests/emu/skip_hooks.cu — test hooks of the P-skip test for the host emulation build (TEST INFRASTRUCTURE ONLY).
-// Linked with emu.cu into the libraries tests/test_gpu_skip_stage.py and tests/test_gpu_skip_decision.py build; the counters are the host build's
-// (enc_inter.cuh: g_skip_outcome, g_skip_phase_luma / g_skip_phase_chroma), filled by every emu_encode.
+// tests/emu/skip_hooks.cu — test hooks of the P-skip test for the host emulation build (TEST INFRASTRUCTURE ONLY).  The counters
+// are the host build's (enc_inter.cuh: g_skip_outcome, g_skip_phase_luma / g_skip_phase_chroma), filled by every emu_encode.
 #include <stdint.h>
 #include <string.h>
 #include <vector>
 
-#include "../../openh264_b200/csrc/enc_frame.cuh"
+#include "../../openh264_b200/csrc/stage_hooks.cuh"
 
 using namespace mbk;
 
@@ -24,53 +23,16 @@ extern "C" int emu_skip_outcomes(uint64_t* out, int n) {
   out[SKIP_OUTCOMES + 1] = g_skip_phase_chroma;
   return SKIP_OUTCOMES + 2;
 }
-// The host build of stage A's P-skip test (fill_inter_cache, predict_sad_skip, pskip_enc) with the job and output layout of
-// the device hook b2h264_debug_skip_test (enc_kernels.cu); planes: HOST memory, the one set every job reads.  Each job's
-// outcome is counted like an encode's (emu_skip_outcomes).
+// The host build of the device hook b2h264_debug_skip_test (enc_kernels.cu), same arguments and refusals; planes: HOST memory,
+// the one set every job reads.  Each job's outcome is counted like an encode's (emu_skip_outcomes).
 extern "C" int emu_skip_test(int n, const uint8_t* planes, long long set_bytes, const uint8_t* jobs, uint8_t* out) {
-  const int in_bytes = 32 * 4 + 384, out_bytes = 8 * 4 + 384;
-  const int32_t unset = 0x5a5a5a5a;
-  if (n < 1 || !planes || !jobs || !out || set_bytes <= 0) return -1;
+  if (!skip_test_args_ok(n, planes, set_bytes, jobs, out)) return -1;
   b2h264_build_host_tables();
   static MbScratch s;
   for (int i = 0; i < n; i++) {
-    const uint8_t* jb = jobs + (size_t)in_bytes * i;
-    const int32_t* J = reinterpret_cast<const int32_t*>(jb);
-    if (J[6] < 0 || J[6] > 51 || J[4] < 0 || J[4] >= J[0] || J[5] < 0 || J[5] >= J[1]) return -1;
     memset(&s, 0, sizeof(s));
-    memcpy(s.cur_y, jb + 128, 256);
-    memcpy(s.cur_c, jb + 384, 128);
-    for (int k = 0; k < 4; k++) {
-      const int32_t* N = J + 12 + 5 * k;
-      s.nbi[k].mb_type = (uint8_t)N[0];
-      for (int b = 0; b < 16; b++) { s.nbi[k].mv[b][0] = (int16_t)N[1]; s.nbi[k].mv[b][1] = (int16_t)N[2]; }
-      s.nb_sad[k] = N[3];
-      s.nb_skip_sad[k] = N[4];
-    }
-    s.col.mb_type = (uint8_t)J[10];
-    s.col.skip_sad = J[11];
-    EncFrameParams p;
-    EncFramePtrs f;
-    memset(&p, 0, sizeof(p));
-    memset(&f, 0, sizeof(f));
-    p.mb_w = J[0]; p.mb_h = J[1]; p.rec_stride_y = J[2]; p.rec_stride_c = J[3]; p.qp = J[6]; p.fast_mode = J[7]; p.ref_is_p = J[9];
-    const size_t cb = (size_t)p.rec_stride_y * (16 * p.mb_h + 64), cr = cb + (size_t)p.rec_stride_c * (8 * p.mb_h + 32);
-    if ((long long)(cr + (size_t)p.rec_stride_c * (8 * p.mb_h + 32)) > set_bytes) return -1;
-    f.ref[0] = planes + (size_t)32 * p.rec_stride_y + 32;
-    f.ref[1] = planes + cb + (size_t)16 * p.rec_stride_c + 16;
-    f.ref[2] = planes + cr + (size_t)16 * p.rec_stride_c + 16;
-    std::vector<int32_t> sad((size_t)p.mb_w * p.mb_h, unset);
-    f.sad_cost = sad.data();
-    mb_ctx(s.ctx, p, f, J[4], J[5]);
-    s.ctx.nb = J[8];
-    const MbCtx& c = s.ctx;
-    fill_inter_cache(c, s);
-    const int sad_pred = predict_sad_skip(s);
-    const SkipResult r = pskip_enc(c, s, sad_pred);
-    int32_t* o = reinterpret_cast<int32_t*>(out + (size_t)out_bytes * i);
-    o[0] = r.ok; o[1] = r.mvx; o[2] = r.mvy; o[3] = sad_pred; o[4] = r.cost_luma; o[5] = r.cost_skip;
-    o[6] = sad[J[5] * p.mb_w + J[4]]; o[7] = 0;
-    memcpy(out + (size_t)out_bytes * i + 32, s.skip_pred, 384);
+    int32_t sad = kSkipSadUnset;
+    skip_test_case(jobs + (size_t)kSkipJobIn * i, planes, &sad, out + (size_t)kSkipJobOut * i, s);
   }
   return 0;
 }

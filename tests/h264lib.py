@@ -175,6 +175,38 @@ def build_oracle():
 
 _oracle = None
 _ref = None
+_emu = None
+
+
+def emu():
+    """tests/emu/libb2h264_emu.so, the host emulation build of the device macroblock code with every stage's test hooks, built
+    (make) and loaded once per process.  The library is shared: a test that depends on its settings (emu_set_*) or counters
+    sets or resets them itself."""
+    global _emu
+    if _emu is None:
+        subprocess.check_call(["make", "-s", "-C", os.path.join(ROOT, "tests", "emu")])
+        E = C.CDLL(os.path.join(ROOT, "tests", "emu", "libb2h264_emu.so"))
+        vp, i = C.c_void_p, C.c_int
+        E.emu_encode.restype = C.c_long
+        E.emu_encode.argtypes = [vp, i, i, i, i, C.c_float, vp, C.c_long, vp, vp]
+        E.emu_stages_run.restype = C.c_uint
+        E.emu_decode.restype = C.c_int
+        E.emu_decode.argtypes = [vp, C.c_long, vp, C.c_long, C.POINTER(i), C.POINTER(i)]
+        E.b2h264_dec_wp_stats.restype = C.c_int
+        E.b2h264_dec_wp_stats.argtypes = [C.POINTER(C.c_longlong), i, i]
+        E.emu_deblock_picture.restype = C.c_int
+        E.emu_deblock_picture.argtypes = [vp] * 3 + [i] * 4 + [vp, vp] + [i] * 4
+        E.emu_decode_records.argtypes = [i, i, i, vp, vp, vp, vp, i, vp, vp, vp]
+        E.emu_skip_test.argtypes = [i, vp, C.c_longlong, vp, vp]
+        E.emu_skip_outcomes.argtypes = [vp, i]
+        E.emu_check_chroma_pair.restype = C.c_long
+        E.emu_me_partitions.argtypes = [i, vp, C.c_longlong, vp, vp]
+        E.emu_intra_tail.argtypes = [i, vp, vp]
+        E.emu_i4_ends.argtypes = [vp, i]
+        E.emu_inter_residual.argtypes = [i, vp, vp, vp]
+        E.emu_res_outcomes.argtypes = [vp, i]
+        _emu = E
+    return _emu
 
 
 def oracle():

@@ -9,8 +9,6 @@ cost limits below, at and above the I4x4 running total (taken from a run without
 complete and lose, and complete and win.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
@@ -159,22 +157,6 @@ def with_limits(base, kinds, qps, run):
             ek.append(kinds[i])
             eq.append(qps[i])
     return np.concatenate([base, np.stack(extra)]), np.concatenate([kinds, ek]), np.concatenate([qps, eq])
-
-
-def build_emu(tmpdir):
-    """the host emulation build (tests/emu/Makefile's sources and flags) with the intra tail's hooks
-    (tests/emu/intra_tail_hooks.cu), compiled into tmpdir"""
-    src = os.path.join(ROOT, "openh264_b200", "csrc")
-    lib = os.path.join(str(tmpdir), "libb2h264_emu_intra_mb.so")
-    subprocess.check_call([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17",
-                           "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "-shared", "-o", lib,
-                           "emu.cu", "emu_tables.cu", "intra_tail_hooks.cu"] +
-                          [os.path.join(src, f) for f in ("h264_bitstream.cpp", "h264_cabac.cpp", "enc_host.cpp", "h264_parse.cpp")],
-                          cwd=os.path.join(ROOT, "tests", "emu"))
-    E = C.CDLL(lib)
-    E.emu_intra_tail.argtypes = [C.c_int, C.c_void_p, C.c_void_p]
-    E.emu_i4_ends.argtypes = [C.c_void_p, C.c_int]
-    return E
 
 
 def run_emu(emu, cases):

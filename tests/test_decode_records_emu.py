@@ -8,8 +8,6 @@ tests/test_gpu_decode_records.py holds the device kernel to the same oracle.  Th
 decoder: on seeded random Baseline streams written with the loop filter off it must reproduce the reference's pictures
 (skipped where the reference build, oracle/_ref, is absent)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -23,19 +21,8 @@ CASES = drc.cases()
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    # the host emulation build (tests/emu/Makefile's sources and flags) plus the construct stage's hook
-    src = os.path.join(ROOT, "openh264_b200", "csrc")
-    lib = str(tmp_path_factory.mktemp("emu_dec_records") / "libb2h264_emu_dec_records.so")
-    subprocess.check_call([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17",
-                           "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "-shared", "-o", lib,
-                           "emu.cu", "emu_tables.cu", "decode_records_hooks.cu"] +
-                          [os.path.join(src, f) for f in ("h264_bitstream.cpp", "h264_cabac.cpp", "enc_host.cpp", "h264_parse.cpp")],
-                          cwd=os.path.join(ROOT, "tests", "emu"))
-    E = C.CDLL(lib)
-    E.emu_decode_records.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
-                                     C.c_void_p, C.c_void_p]
-    return E
+def emu():
+    return h264lib.emu()
 
 
 def padded_bytes(mb_w, mb_h):

@@ -6,7 +6,6 @@ records, then the same deblocking code the encoder path uses) behind the host bi
 The device kernel that batches this stage does not exist yet; the product decoder entry points still fail loudly."""
 import ctypes as C
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -19,11 +18,7 @@ ROOT = h264lib.ROOT
 
 @pytest.fixture(scope="module")
 def emu():
-    subprocess.check_call(["make", "-s", "-C", os.path.join(ROOT, "tests", "emu")])
-    E = C.CDLL(os.path.join(ROOT, "tests", "emu", "libb2h264_emu.so"))
-    E.emu_decode.restype = C.c_int
-    E.emu_decode.argtypes = [C.c_void_p, C.c_long, C.c_void_p, C.c_long, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    return E
+    return h264lib.emu()
 
 
 def ref_decode(bs):
@@ -193,15 +188,14 @@ def test_host_decoder_cabac_streams_of_our_encoder(emu):
     """the host build of the encoder writes the same pictures with CAVLC and with CABAC (High and Main parameter sets): the CABAC
     parser + construct path must give the encoder's own reconstruction, i.e. the same pictures as the CAVLC stream decodes to —
     and what the reference decoder makes of the CABAC stream where it is available"""
-    emu.emu_encode.restype = C.c_long
-    emu.emu_encode.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_long, C.c_void_p, C.c_void_p]
-    emu.emu_decode.argtypes = [C.c_void_p, C.c_long, C.c_void_p, C.c_long, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     for (w, h, n, qp, seed, noise) in [(176, 144, 5, 24, 3, 3), (320, 192, 4, 33, 5, 12), (64, 48, 4, 8, 6, 30), (180, 148, 4, 40, 9, 3)]:
         yuv = h264lib.synth_clip(w, h, n, seed=seed, noise=noise)
         pics = []
         for entropy in ((0, 66), (1, 0), (1, 77)):
             emu.emu_set_complexity_low(0)
             emu.emu_set_entropy(*entropy)
+            emu.emu_set_intra_period(0)
+            emu.emu_set_loop_filter(0, 0, 0)
             bs, fb, rec = np.zeros(16 << 20, np.uint8), np.zeros(n, np.int32), np.zeros(yuv.size, np.uint8)
             tot = emu.emu_encode(yuv.ctypes.data, w, h, n, qp, 30.0, bs.ctypes.data, bs.size, fb.ctypes.data, rec.ctypes.data)
             assert tot > 0

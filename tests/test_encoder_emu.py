@@ -4,11 +4,9 @@ bitstream bit for bit — against the golden SHA-1s generated from the reference
 reference_clips.json: incl. the reference's own res/CiscoVT2people_320x192_12fps.yuv clip, BASELINE.json config 2) and,
 where oracle/_ref exists, against the reference run side by side.  The GPU build of the same source is
 checked by tests/test_gpu_encoder.py."""
-import ctypes as C
 import hashlib
 import json
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -36,12 +34,7 @@ def check_reference_clip(emu, name, w, h, n, qp, fps, entropy=(0, 66)):
 
 @pytest.fixture(scope="module")
 def emu():
-    subprocess.check_call(["make", "-s", "-C", os.path.join(ROOT, "tests", "emu")])
-    E = C.CDLL(os.path.join(ROOT, "tests", "emu", "libb2h264_emu.so"))
-    E.emu_encode.restype = C.c_long
-    E.emu_encode.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_long, C.c_void_p, C.c_void_p]
-    E.emu_stages_run.restype = C.c_uint
-    return E
+    return h264lib.emu()
 
 
 def emu_encode(E, yuv, w, h, n, qp, fps, low=False, entropy=(0, 66), intra_period=0, loop_filter=(0, 0, 0)):

@@ -29,14 +29,7 @@ STATS = ["one list L0", "one list L1", "two lists 16x16", "two lists 16x8", "two
 
 @pytest.fixture(scope="module")
 def emu():
-    import subprocess
-    subprocess.check_call(["make", "-s", "-C", os.path.join(ROOT, "tests", "emu")])
-    E = C.CDLL(os.path.join(ROOT, "tests", "emu", "libb2h264_emu.so"))
-    E.emu_decode.restype = C.c_int
-    E.emu_decode.argtypes = [C.c_void_p, C.c_long, C.c_void_p, C.c_long, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    E.b2h264_dec_wp_stats.restype = C.c_int
-    E.b2h264_dec_wp_stats.argtypes = [C.POINTER(C.c_longlong), C.c_int, C.c_int]
-    return E
+    return h264lib.emu()
 
 
 def source(name):

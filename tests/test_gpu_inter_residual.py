@@ -8,7 +8,6 @@ import ctypes as C
 import hashlib
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -27,21 +26,8 @@ OUTCOMES = ["luma levels dropped by ctr_mb < 6", "kept and dropped 8x8 in one ma
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    # the host emulation build (tests/emu/Makefile's sources and flags) plus this step's hooks (tests/emu/inter_residual_hooks.cu)
-    src = os.path.join(ROOT, "openh264_b200", "csrc")
-    lib = str(tmp_path_factory.mktemp("emu_res") / "libb2h264_emu_res.so")
-    subprocess.check_call([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17",
-                           "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "-shared", "-o", lib,
-                           "emu.cu", "emu_tables.cu", "inter_residual_hooks.cu"] +
-                          [os.path.join(src, f) for f in ("h264_bitstream.cpp", "h264_cabac.cpp", "enc_host.cpp", "h264_parse.cpp")],
-                          cwd=os.path.join(ROOT, "tests", "emu"))
-    E = C.CDLL(lib)
-    E.emu_encode.restype = C.c_long
-    E.emu_encode.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_long, C.c_void_p, C.c_void_p]
-    E.emu_inter_residual.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    E.emu_res_outcomes.argtypes = [C.c_void_p, C.c_int]
-    return E
+def emu():
+    return h264lib.emu()
 
 
 def make_cases():
@@ -195,7 +181,18 @@ def test_device_pass_matches_host_build(emu):
     assert L.b2h264_debug_inter_residual(len(qp), src.ctypes.data, qp.ctypes.data, got.ctypes.data) == 0
     bad = np.nonzero((got != want).any(1))[0]
     assert len(bad) == 0, f"{len(bad)} of {len(qp)} cases differ, first: case {bad[0]} qp {qp[bad[0]]}"
-    # bad arguments are refused before anything is launched
+    _refusals(L.b2h264_debug_inter_residual)
+
+
+def test_host_build_refuses_bad_arguments(emu):
+    """the host build refuses what the device hook refuses (stage_hooks.cuh: inter_residual_args_ok)"""
+    _refusals(emu.emu_inter_residual)
+
+
+def _refusals(fn):
+    # bad arguments are refused before anything runs
+    src, qp = make_cases()
+    got = np.zeros((1, OUT_BYTES), np.uint8)
     q = np.array([52], np.int32)
-    assert L.b2h264_debug_inter_residual(1, src.ctypes.data, q.ctypes.data, got.ctypes.data) == -1
-    assert L.b2h264_debug_inter_residual(0, src.ctypes.data, qp.ctypes.data, got.ctypes.data) == -1
+    assert fn(1, src.ctypes.data, q.ctypes.data, got.ctypes.data) == -1
+    assert fn(0, src.ctypes.data, qp.ctypes.data, got.ctypes.data) == -1

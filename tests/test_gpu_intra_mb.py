@@ -9,14 +9,15 @@ import os
 import numpy as np
 import pytest
 
+import h264lib
 import intra_mb_cases as ic
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "intra_mb.json")
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    return ic.build_emu(tmp_path_factory.mktemp("emu_intra_mb"))
+def emu():
+    return h264lib.emu()
 
 
 @pytest.mark.gpu

@@ -6,8 +6,6 @@ I4x4 modes and their prev / rem flags, I16x16 and chroma modes), reconstruction 
 structured macroblocks at QP 0 / 12 / 26 / 40 / 51, every neighbour-availability nibble, HIGH and LOW complexity, and cost
 limits placed around the I4x4 running total so that the loop breaks early, completes and loses, or completes and wins."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -25,19 +23,8 @@ I4_END = ["I4x4 loop broke early", "I4x4 loop completed", "I4x4 won"]   # enc_mb
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    # the host emulation build (tests/emu/Makefile's sources and flags) plus the tail's hooks (tests/emu/intra_tail_hooks.cu)
-    src = os.path.join(ROOT, "openh264_b200", "csrc")
-    lib = str(tmp_path_factory.mktemp("emu_tail") / "libb2h264_emu_tail.so")
-    subprocess.check_call([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17",
-                           "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "-shared", "-o", lib,
-                           "emu.cu", "emu_tables.cu", "intra_tail_hooks.cu"] +
-                          [os.path.join(src, f) for f in ("h264_bitstream.cpp", "h264_cabac.cpp", "enc_host.cpp", "h264_parse.cpp")],
-                          cwd=os.path.join(ROOT, "tests", "emu"))
-    E = C.CDLL(lib)
-    E.emu_intra_tail.argtypes = [C.c_int, C.c_void_p, C.c_void_p]
-    E.emu_i4_ends.argtypes = [C.c_void_p, C.c_int]
-    return E
+def emu():
+    return h264lib.emu()
 
 
 def content(rng, kind, h, w):
@@ -174,8 +161,19 @@ def test_device_tail_matches_host_build(emu):
     bad = np.nonzero((got != want).any(1))[0]
     assert len(bad) == 0, f"{len(bad)} of {len(cases)} cases differ, first: case {bad[0]}, bytes " \
                           f"{np.nonzero(got[bad[0]] != want[bad[0]])[0][:16].tolist()}"
-    # bad arguments are refused before anything is launched
-    c = cases[:1].copy()
+    _refusals(L.b2h264_debug_intra_tail)
+
+
+def test_host_build_refuses_bad_arguments(emu):
+    """the host build refuses what the device hook refuses (stage_hooks.cuh: intra_tail_args_ok)"""
+    _refusals(emu.emu_intra_tail)
+
+
+def _refusals(fn):
+    # bad arguments are refused before anything runs
+    c = base_cases()[:1].copy()
+    got = np.zeros((1, OUT_BYTES), np.uint8)
+    assert fn(1, c.ctypes.data, got.ctypes.data) == 0
+    assert fn(0, c.ctypes.data, got.ctypes.data) == -1
     c[0, TILE + 384:TILE + 388] = np.array([52], np.int32).view(np.uint8)
-    assert L.b2h264_debug_intra_tail(1, c.ctypes.data, got.ctypes.data) == -1
-    assert L.b2h264_debug_intra_tail(0, cases.ctypes.data, got.ctypes.data) == -1
+    assert fn(1, c.ctypes.data, got.ctypes.data) == -1

@@ -18,8 +18,6 @@ uses, so only three or four columns short would a wrong choice show) and from th
 refinement; all quarter-sample phases the refinement can end on (the centre (2, 2) and the diagonals (1|3, 1|3) are not
 among its candidates) and the chroma eighth-sample phases that follow, for 4- and 8-wide chroma blocks."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -41,18 +39,8 @@ REFINE_PHASES = {(0, 0), (2, 0), (0, 2), (1, 0), (3, 0), (0, 1), (0, 3), (2, 1),
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    # the host emulation build (tests/emu/Makefile's sources and flags) plus the search hooks (tests/emu/me_hooks.cu)
-    src = os.path.join(ROOT, "openh264_b200", "csrc")
-    lib = str(tmp_path_factory.mktemp("emu_me") / "libb2h264_emu_me.so")
-    subprocess.check_call([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17",
-                           "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "-shared", "-o", lib,
-                           "emu.cu", "emu_tables.cu", "me_hooks.cu"] +
-                          [os.path.join(src, f) for f in ("h264_bitstream.cpp", "h264_cabac.cpp", "enc_host.cpp", "h264_parse.cpp")],
-                          cwd=os.path.join(ROOT, "tests", "emu"))
-    E = C.CDLL(lib)
-    E.emu_me_partitions.argtypes = [C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p]
-    return E
+def emu():
+    return h264lib.emu()
 
 
 # ---- pictures ------------------------------------------------------------------------------------------------------
@@ -477,23 +465,40 @@ def test_device_matches_host_build(dev, emu):
 @pytest.mark.gpu
 def test_device_refuses_bad_arguments(dev):
     L, m = dev
+    pic, _ = cases()[2]
+    planes = m.DeviceArray(np.tile(pic.set, 2))
+    call = _refusals(lambda n, set_bytes, jobs, out: L.b2h264_debug_me_partitions(n, planes.ptr, set_bytes, jobs, 1, out))
+    # device only: one tensor map covers every job's planes, and the window copy needs 16- / 8-byte aligned rows
+    assert call(2, pic.sy + 8) and call(3, pic.sc + 4)                 # strides: luma not a multiple of 16, chroma of 8
+    assert call(None, 0, set_bytes=len(pic.set) + 8)                   # sets not on 16-byte boundaries
+
+
+def test_host_build_refuses_bad_arguments(emu):
+    """the host build refuses what both builds refuse (stage_hooks.cuh: me_partitions_args_ok)"""
+    pic, _ = cases()[2]
+    planes = np.tile(pic.set, 2)
+    _refusals(lambda n, set_bytes, jobs, out: emu.emu_me_partitions(n, planes.ctypes.data, set_bytes, jobs, out))
+
+
+def _refusals(fn):
+    """the refusals both builds share; fn(n, set_bytes, jobs, out) runs one build's hook on two plane sets.  Returns the refused()
+    check for the caller's own rules."""
     pic, jobs = cases()[2]
     good = np.stack([record(pic, j) for j in jobs[:2]])
-    planes = m.DeviceArray(np.tile(pic.set, 2))
     out = np.zeros((2, OUT_BYTES), np.uint8)
     n_set = len(pic.set)
-    assert L.b2h264_debug_me_partitions(2, planes.ptr, n_set, good.ctypes.data, 1, out.ctypes.data) == 0
+    assert fn(2, n_set, good.ctypes.data, out.ctypes.data) == 0
 
     def refused(word, value, n=2, set_bytes=n_set):
         bad = good.copy()
         if word is not None:
             bad[1, 4 * word:4 * word + 4] = np.array([value], np.int32).view(np.uint8)
-        return L.b2h264_debug_me_partitions(n, planes.ptr, set_bytes, bad.ctypes.data, 1, out.ctypes.data) == -1
+        return fn(n, set_bytes, bad.ctypes.data, out.ctypes.data) == -1
     assert refused(7, 52) and refused(7, -1)                           # QP
     assert refused(5, pic.mb_w) and refused(6, pic.mb_h) and refused(5, -1)   # macroblock outside the picture
-    assert refused(2, pic.sy + 8) and refused(3, pic.sc + 4)           # strides: luma not a multiple of 16, chroma of 8
     assert refused(2, pic.sy - 16)                                     # narrower than the padded picture
     assert refused(4, -1)                                              # negative mv_range: blocks could leave the padding
     assert refused(11, 4) and refused(14, 6)                           # shape, candidate count
-    assert refused(None, 0, set_bytes=n_set - 16) and refused(None, 0, set_bytes=n_set + 8)
+    assert refused(None, 0, set_bytes=n_set - 16)
     assert refused(None, 0, n=0)
+    return refused

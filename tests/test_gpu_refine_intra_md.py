@@ -2,11 +2,9 @@
 quarter-sample offsets (tests/golden/make_refine_intra_golden.py): the host emulation build and the GPU encoder, with
 batches of sms // 2 + 1 streams, must reproduce the reference encoder's bitstream in complexity HIGH and LOW at QP 12,
 26 and 40 (golden = the unmodified reference, tests/golden/refine_intra.json)."""
-import ctypes as C
 import hashlib
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -36,11 +34,7 @@ def clip(key):
 
 @pytest.fixture(scope="module")
 def emu():
-    subprocess.check_call(["make", "-s", "-C", os.path.join(ROOT, "tests", "emu")])
-    E = C.CDLL(os.path.join(ROOT, "tests", "emu", "libb2h264_emu.so"))
-    E.emu_encode.restype = C.c_long
-    E.emu_encode.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_long, C.c_void_p, C.c_void_p]
-    return E
+    return h264lib.emu()
 
 
 @pytest.mark.parametrize("key", sorted(GOLD))

@@ -15,8 +15,6 @@ eighth-sample chroma phase at every chroma alignment, the range guard's limits f
 vector's derivation, the early accepts exactly at their boundaries, the largest packed SAD, the residual scores exactly at
 their thresholds, and every QP in both complexity modes."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -34,19 +32,8 @@ O = {name: k for k, name in enumerate(h264lib.PSKIP_OUTCOMES)}
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    # the host emulation build (tests/emu/Makefile's sources and flags) plus the skip test's hooks (tests/emu/skip_hooks.cu)
-    src = os.path.join(ROOT, "openh264_b200", "csrc")
-    lib = str(tmp_path_factory.mktemp("emu_skip_decision") / "libb2h264_emu_skip_decision.so")
-    subprocess.check_call([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17",
-                           "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "-shared", "-o", lib,
-                           "emu.cu", "emu_tables.cu", "skip_hooks.cu"] +
-                          [os.path.join(src, f) for f in ("h264_bitstream.cpp", "h264_cabac.cpp", "enc_host.cpp", "h264_parse.cpp")],
-                          cwd=os.path.join(ROOT, "tests", "emu"))
-    E = C.CDLL(lib)
-    E.emu_skip_test.argtypes = [C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p]
-    E.emu_skip_outcomes.argtypes = [C.c_void_p, C.c_int]
-    return E
+def emu():
+    return h264lib.emu()
 
 
 # ---- pictures ------------------------------------------------------------------------------------------------------
@@ -538,17 +525,26 @@ def test_device_matches_host_build(dev, emu):
 
 @pytest.mark.gpu
 def test_device_refuses_bad_arguments(dev):
+    _refusals(dev.b2h264_debug_skip_test)
+
+
+def test_host_build_refuses_bad_arguments(emu):
+    """the host build refuses what the device hook refuses (stage_hooks.cuh: skip_test_args_ok)"""
+    _refusals(emu.emu_skip_test)
+
+
+def _refusals(fn):
     pic, jobs = cases()[1]
     good = np.stack([record(pic, j) for j in jobs[:2]])
     out = np.zeros((2, OUT_BYTES), np.uint8)
     n_set = len(pic.set)
-    assert dev.b2h264_debug_skip_test(2, pic.set.ctypes.data, n_set, good.ctypes.data, out.ctypes.data) == 0
+    assert fn(2, pic.set.ctypes.data, n_set, good.ctypes.data, out.ctypes.data) == 0
 
     def refused(word, value, n=2, set_bytes=n_set):
         bad = good.copy()
         if word is not None:
             bad[1, 4 * word:4 * word + 4] = np.array([value], np.int32).view(np.uint8)
-        return dev.b2h264_debug_skip_test(n, pic.set.ctypes.data, set_bytes, bad.ctypes.data, out.ctypes.data) == -1
+        return fn(n, pic.set.ctypes.data, set_bytes, bad.ctypes.data, out.ctypes.data) == -1
     assert refused(6, 52) and refused(6, -1)                           # QP
     assert refused(4, pic.mb_w) and refused(5, pic.mb_h) and refused(4, -1) and refused(5, -1)   # macroblock outside the picture
     assert refused(2, pic.sy - 1) and refused(3, pic.sc - 1)           # strides narrower than the padded picture

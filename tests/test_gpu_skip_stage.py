@@ -4,11 +4,9 @@ each test decide.  The host emulation build and the GPU encoder, with batches of
 reference encoder's bitstream in complexity HIGH and LOW at QP 12, 26 and 40 (golden = the unmodified reference,
 tests/golden/skip_stage.json); the host build also counts which outcome each skip test had.  The packed chroma
 prediction is checked against the per-sample one for every phase and block size."""
-import ctypes as C
 import hashlib
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -39,21 +37,8 @@ def clip(key):
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    # the host emulation build (tests/emu/Makefile's sources and flags) plus the skip test's hooks (tests/emu/skip_hooks.cu)
-    src = os.path.join(ROOT, "openh264_b200", "csrc")
-    lib = str(tmp_path_factory.mktemp("emu_skip") / "libb2h264_emu_skip.so")
-    subprocess.check_call([os.environ.get("NVCC", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17",
-                           "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "-shared", "-o", lib,
-                           "emu.cu", "emu_tables.cu", "skip_hooks.cu"] +
-                          [os.path.join(src, f) for f in ("h264_bitstream.cpp", "h264_cabac.cpp", "enc_host.cpp", "h264_parse.cpp")],
-                          cwd=os.path.join(ROOT, "tests", "emu"))
-    E = C.CDLL(lib)
-    E.emu_encode.restype = C.c_long
-    E.emu_encode.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_long, C.c_void_p, C.c_void_p]
-    E.emu_skip_outcomes.argtypes = [C.c_void_p, C.c_int]
-    E.emu_check_chroma_pair.restype = C.c_long
-    return E
+def emu():
+    return h264lib.emu()
 
 
 def emu_encode(emu, key):

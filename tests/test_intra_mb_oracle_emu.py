@@ -19,8 +19,8 @@ I4_END = ["broke early", "completed and lost", "completed and won"]
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    return ic.build_emu(tmp_path_factory.mktemp("emu_intra_mb"))
+def emu():
+    return h264lib.emu()
 
 
 @pytest.fixture(scope="module")
