@@ -15,7 +15,7 @@
  * 1-stream layer-2 encoder.
  *
  * Supported configuration (everything else is rejected with an error, never silently approximated):
- * CAMERA_VIDEO_REAL_TIME, 1 spatial / 1 temporal layer, RC_OFF_MODE (constant QP), SM_SINGLE_SLICE,
+ * CAMERA_VIDEO_REAL_TIME, 1 spatial / 1 temporal layer, RC_OFF_MODE (constant QP), SM_SINGLE_SLICE, SM_FIXEDSLCNUM_SLICE or SM_RASTER_SLICE,
  * CAVLC or CABAC (Baseline / Main / High parameter sets, no 8x8 transform), any iComplexityMode (LOW / MEDIUM / HIGH), 1 reference frame, any loop filter idc / offsets, IDR at the first frame, every uiIntraPeriod frames and on
  * ForceIntraFrame, no denoise / background detection / scene-change / LTR.  (Adaptive quantisation: the reference switches it off
  * for every configuration, encoder_ext.cpp:300-301, so its output with the flag set is this constant-QP output.)
@@ -49,7 +49,7 @@ typedef struct {
                                  * count as unspecified.  No High-profile tool is used (no 8x8 transform): only the SPS / PPS change */
   int32_t intra_period;         /* SEncParamExt::uiIntraPeriod: 0 = only the first picture (and forced ones) is IDR; N: a stream codes an
                                  * IDR picture once N - 1 P pictures followed the last one (wels_preprocess.cpp:369-371) */
-  int32_t loop_filter_idc;      /* iLoopFilterDisableIdc: 0 on, 1 off, 2 = 0 (one slice per picture) */
+  int32_t loop_filter_idc;      /* iLoopFilterDisableIdc: 0 on, 1 off, 2 on except at slice edges (= 0 with one slice per picture) */
   int32_t loop_filter_alpha_c0_offset, loop_filter_beta_offset;   /* iLoopFilterAlphaC0Offset / iLoopFilterBetaOffset, -6..6 */
 } b2h264_enc_config;
 
@@ -85,6 +85,18 @@ int  b2h264_enc_force_idr (b2h264_enc* e, int stream);
  * b2h264_enc_get_references: out4 = iNumRefFrame and max_num_ref_frames as resolved, iLTRRefNum, pictures kept per stream. */
 int  b2h264_enc_set_references (b2h264_enc* e, int num_ref_frames, int ltr_enable, int ltr_mark_period);
 int  b2h264_enc_get_references (b2h264_enc* e, int32_t* out4);
+
+/* Slices, before the first submit (-3 after it; -2 for a request that is refused).  mode, num and mb_num are SSliceArgument's
+ * uiSliceMode, uiSliceNum and uiSliceMbNum (35 entries, or NULL for zeros), resolved as the reference resolves them
+ * (encoder_ext.cpp:173-250,540-612): SM_SINGLE_SLICE (0); SM_FIXEDSLCNUM_SLICE (1): num slices of floor(macroblocks / num)
+ * macroblocks, the last one taking the remainder, num clamped to 35; SM_RASTER_SLICE (2): mb_num[0] == 0 codes one slice per
+ * macroblock row (refused with more than 35 rows), otherwise the runs of mb_num, the last one cut or a remainder added.  A
+ * picture of at most 48 macroblocks, or a request for one slice, falls back to SM_SINGLE_SLICE.  Refused: SM_SIZELIMITED_SLICE,
+ * and SM_FIXEDSLCNUM_SLICE with num 0 (the reference takes the CPU core count).  All streams of the encoder share the
+ * partition.  Each slice is one NAL unit; with several slices loop_filter_idc 2 leaves the edges between slices unfiltered.
+ * b2h264_enc_get_slices: the resolved mode, slice count and run lengths (any pointer may be NULL). */
+int  b2h264_enc_set_slices (b2h264_enc* e, int mode, int num, const uint32_t* mb_num);
+int  b2h264_enc_get_slices (b2h264_enc* e, int32_t* mode, int32_t* num, uint32_t* mb_num);
 
 /* Loss-recovery feedback of stream i (SLTRRecoverRequest / SLTRMarkingFeedback of ENCODER_LTR_RECOVERY_REQUEST /
  * ENCODER_LTR_MARKING_FEEDBACK; feedback_type 1 = LTR_RECOVERY_REQUEST, 4 / 5 = LTR_MARKING_SUCCESS / _FAILED).  It takes

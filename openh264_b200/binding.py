@@ -93,6 +93,8 @@ API = {
     "b2h264_enc_get_recon": [vp, C.c_int, vp],
     "b2h264_enc_set_references": [vp, C.c_int, C.c_int, C.c_int],
     "b2h264_enc_get_references": [vp, i32p],
+    "b2h264_enc_set_slices": [vp, C.c_int, C.c_int, C.POINTER(C.c_uint32)],
+    "b2h264_enc_get_slices": [vp, i32p, i32p, C.POINTER(C.c_uint32)],
     "b2h264_enc_ltr_recovery_request": [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int],
     "b2h264_enc_ltr_marking_feedback": [vp, C.c_int, C.c_int, C.c_int, C.c_int],
     "b2h264_enc_ltr_mark_period": [vp, C.c_int, C.c_int],
@@ -230,6 +232,16 @@ class BatchEncoder:
         v = (C.c_int32 * 4)()
         check(self.L.b2h264_enc_get_references(self.h, v))
         return tuple(v)
+
+    def set_slices(self, mode, num=1, mb_num=()):
+        """Slices of every picture of every stream, before the first picture: SSliceArgument's uiSliceMode (0 SM_SINGLE_SLICE,
+        1 SM_FIXEDSLCNUM_SLICE, 2 SM_RASTER_SLICE), uiSliceNum and uiSliceMbNum (up to 35 run lengths; none with raster mode: one
+        slice per macroblock row).  Returns the partition as the reference resolves it: (mode, slice count, run lengths)."""
+        runs = (C.c_uint32 * 35)(*mb_num)
+        check(self.L.b2h264_enc_set_slices(self.h, mode, num, runs))
+        m, n = C.c_int32(), C.c_int32()
+        check(self.L.b2h264_enc_get_slices(self.h, C.byref(m), C.byref(n), runs))
+        return m.value, n.value, list(runs[:n.value]) if m.value else []
 
     def ltr_recovery_request(self, stream, idr_pic_id, cur_frame_num, last_correct_frame_num, feedback_type=1):
         """ENCODER_LTR_RECOVERY_REQUEST for one stream (feedback_type 1 = LTR_RECOVERY_REQUEST); applies to its next picture"""

@@ -15,6 +15,7 @@
 #include "cuda_owned.h"
 #include "enc_host.h"
 #include "enc_launch.h"
+#include "enc_slices.h"
 #include "host_pool.h"
 
 using b2h264::StreamCtl;
@@ -23,6 +24,7 @@ using b2h264::RefConfig;
 using b2h264::RefDecision;
 using b2h264::Pool;
 using b2h264::PicLayout;
+using b2h264::SliceConfig;
 using b2h264::DeviceBuf;
 using b2h264::HostBuf;
 using b2h264::Event;
@@ -44,6 +46,8 @@ struct b2h264_enc {
   std::vector<int32_t> p_since_idr;       // per stream: P pictures since the last IDR (SSpatialLayerInternal::iFrameIndex)
   std::vector<StreamRefs> refs;           // per stream: reference lists, long-term state, slots of its pictures (enc_refs.h)
   RefConfig refcfg;                       // b2h264_enc_set_references; the default is one reference, no LTR
+  SliceConfig slices;                     // b2h264_enc_set_slices; the default is one slice per picture
+  std::vector<int32_t> slice_first;       // first macroblock of each slice (more than one slice only)
   bool started = false;                   // a picture has been submitted: the picture store is fixed
   // the CUDA resources are released in the reverse order of their declaration: the buffers and events before the streams
   Stream own_st;                          // the encoder's kernel stream until b2h264_enc_set_stream lends it the caller's
@@ -61,6 +65,7 @@ struct b2h264_enc {
   DeviceBuf<MbOut> d_out[2];
   DeviceBuf<int32_t> d_sad;
   DeviceBuf<int32_t> d_bits;              // S x n_mb: exact CAVLC bits per macroblock (when enabled)
+  DeviceBuf<int32_t> d_slice_first;       // n_mb: first macroblock of each macroblock's slice (several slices only; EncFramePtrs)
   bool mb_bits_on = false;
   DeviceBuf<int> d_tickets;
   DeviceBuf<uint8_t> d_stash;             // parked macroblock scratches of the staged scheduler
@@ -100,6 +105,7 @@ struct b2h264_enc {
     c.fast_mode = cfg.complexity_low != 0;
     c.record_mb_bits = mb_bits_on;
     c.set_num_ref_frames(refcfg.sps_num_ref_frames, cfg.target_bitrate);
+    c.slice_first = slice_first;
     return c.set_loop_filter(cfg.loop_filter_idc, cfg.loop_filter_alpha_c0_offset, cfg.loop_filter_beta_offset);
   }
   // allocates the picture store, its co-located records and the source pictures for configuration c, zero-filled, and
@@ -235,6 +241,42 @@ int b2h264_enc_get_references(b2h264_enc* e, int32_t* out4) {
   return 0;
 }
 
+int b2h264_enc_set_slices(b2h264_enc* e, int mode, int num, const uint32_t* mb_num) {
+  if (!e) return -1;
+  SliceConfig c;
+  const char* why = nullptr;
+  if (num < 0 || !SliceConfig::resolve(mode, num, mb_num, e->ctl[0].sp.mb_w, e->ctl[0].sp.mb_h, &c, &why)) return -2;
+  if (e->started) return -3;
+  CK(cudaSetDevice(e->cfg.device));
+  std::vector<int32_t> first(c.slices() + 1);
+  c.starts(e->n_mb, first.data());
+  if (c.slices() > 1) {
+    // every macroblock carries its slice's first address: availability is one load and two compares (enc_frame.cuh: mb_ctx)
+    std::vector<int32_t> per_mb(e->n_mb);
+    for (int k = 0; k < c.slices(); k++)
+      for (int i = first[k]; i < first[k + 1]; i++) per_mb[i] = first[k];
+    DeviceBuf<int32_t> d;
+    CK(d.alloc(e->n_mb * sizeof(int32_t)));
+    CK(cudaMemcpy(d.get(), per_mb.data(), e->n_mb * sizeof(int32_t), cudaMemcpyHostToDevice));
+    e->d_slice_first = std::move(d);
+    first.pop_back();
+    e->slice_first.swap(first);
+  } else {
+    e->slice_first.clear();
+  }
+  e->slices = c;
+  for (int s = 0; s < e->S; s++) e->init_stream(s);   // cannot fail: create accepted the loop-filter values
+  return 0;
+}
+
+int b2h264_enc_get_slices(b2h264_enc* e, int32_t* mode, int32_t* num, uint32_t* mb_num) {
+  if (!e) return -1;
+  if (mode) *mode = e->slices.mode;
+  if (num) *num = e->slices.num;
+  if (mb_num) memcpy(mb_num, e->slices.mb_num, sizeof(e->slices.mb_num));
+  return 0;
+}
+
 int b2h264_enc_ltr_recovery_request(b2h264_enc* e, int stream, int feedback_type, int idr_pic_id, int cur_frame_num,
                                     int last_correct_frame_num) {
   if (!e || stream < 0 || stream >= e->S) return -1;
@@ -327,6 +369,7 @@ int b2h264_enc_submit(b2h264_enc* e, const uint8_t* const* src, int src_on_devic
     F.f.out = e->d_out[k].get() + (size_t)i * e->n_mb;
     F.f.sad_cost = e->d_sad.get() + (size_t)s * e->n_mb;
     F.f.mb_bits = e->mb_bits_on ? e->d_bits.get() + (size_t)s * e->n_mb : nullptr;
+    F.f.slice_first = e->slice_first.empty() ? nullptr : e->d_slice_first.get();
   }
   e->started = true;
   if (!src_on_device) {                        // the kernels of this picture wait for its uploads only

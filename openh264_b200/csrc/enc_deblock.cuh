@@ -214,7 +214,9 @@ template <bool BSL, typename Tile>
 MBK_HD void dbk_filter_store(const EncFrameParams& p, const EncFramePtrs& f, int mbx, int mby, Tile& t) {
   const MbInfo* cur = &t.m[0];
   // decoder: per-slice control travels in MbInfo::p16x16_mv (dec_mb.cuh): disable_deblocking_filter_idc, FilterOffsetA / B and the
-  // slice number (idc 2: edges between slices stay unfiltered).  The encoder path codes one slice: its control is per picture.
+  // slice number (idc 2: edges between slices stay unfiltered).  The encoder's control is per picture, and its slices are raster
+  // runs: a neighbour is in another slice when its address is below the first of the macroblock's slice (EncFramePtrs::slice_first,
+  // present whenever the encoder codes idc 2; bLeftBsValid / bTopBsValid, deblocking.cpp:367-368)
   int idc = p.dbk_idc, off_a = p.dbk_off_a, off_b = p.dbk_off_b;
   if (p.dec_mode) {
     const int v = (uint16_t)cur->p16x16_mv[1];
@@ -222,8 +224,16 @@ MBK_HD void dbk_filter_store(const EncFrameParams& p, const EncFramePtrs& f, int
   }
   if (idc == 1) return;
   // idc 2: edges between slices stay unfiltered
-  const bool have_left = mbx > 0 && !(idc == 2 && t.m[1].p16x16_mv[0] != cur->p16x16_mv[0]);
-  const bool have_top = mby > 0 && !(idc == 2 && t.m[2].p16x16_mv[0] != cur->p16x16_mv[0]);
+  bool cut_left = false, cut_top = false;
+  if (idc == 2) {
+    if (p.dec_mode) { cut_left = t.m[1].p16x16_mv[0] != cur->p16x16_mv[0]; cut_top = t.m[2].p16x16_mv[0] != cur->p16x16_mv[0]; }
+    else {
+      const int idx = mby * p.mb_w + mbx, first = f.slice_first[idx];
+      cut_left = idx - 1 < first; cut_top = idx - p.mb_w < first;
+    }
+  }
+  const bool have_left = mbx > 0 && !cut_left;
+  const bool have_top = mby > 0 && !cut_top;
   [[maybe_unused]] const DecMbAuxB* lb[3] = {nullptr, nullptr, nullptr};
   if constexpr (BSL) if (f.dec_aux_b) {                                         // a picture with B slices: list 1 of the B macroblocks among the three
     constexpr int kWb = (int)(sizeof(DecMbAuxB) / 4);

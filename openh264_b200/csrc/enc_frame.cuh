@@ -19,8 +19,11 @@ MBK_HD void mb_ctx(MbCtx& c, const EncFrameParams& p, const EncFramePtrs& f, int
   for (int i = lane_id(); i < (int)(sizeof(EncFramePtrs) / 4); i += MBK_WS) df[i] = sfp[i];
   if (lane_id() == 0) {
     c.mbx = mbx; c.mby = mby;
-    c.nb = (mbx > 0 ? NB_LEFT : 0) | (mby > 0 ? NB_TOP : 0) | (mbx > 0 && mby > 0 ? NB_TOPLEFT : 0) |
-           (mby > 0 && mbx < p.mb_w - 1 ? NB_TOPRIGHT : 0);
+    // a neighbour is available when it lies in the picture and in the macroblock's slice: slices are raster runs, so when its
+    // address is not below the slice's first (with one slice every neighbour in the picture qualifies)
+    const int idx = mby * p.mb_w + mbx, first = f.slice_first ? f.slice_first[idx] : 0, top = idx - p.mb_w;
+    c.nb = (mbx > 0 && idx - 1 >= first ? NB_LEFT : 0) | (mby > 0 && top >= first ? NB_TOP : 0) |
+           (mbx > 0 && mby > 0 && top - 1 >= first ? NB_TOPLEFT : 0) | (mby > 0 && mbx < p.mb_w - 1 && top + 1 >= first ? NB_TOPRIGHT : 0);
     c.qp = p.qp;
     c.qp_c = tbl_chroma_qp(p.qp);          // chroma_qp_index_offset = 0
     c.lambda = tbl_lambda(p.qp);

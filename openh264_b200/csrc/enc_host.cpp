@@ -130,9 +130,15 @@ void StreamCtl::write_au(bool idr, const MbOut* const* mbs, std::vector<uint8_t>
     ss.n_mmco = refs->n_mmco;
     memcpy(ss.mmco, refs->mmco, sizeof(ss.mmco));
   }
-  if (sp.entropy_cabac) write_slice_cabac(sp, ss, mbs, &rbsp);
-  else write_slice(sp, ss, mbs, &rbsp, record_mb_bits ? &last_mb_bits : nullptr);
-  append_nal(au, 3, idr ? 5 : 1, rbsp);
+  const int n_slices = slice_first.size() < 2 ? 1 : (int)slice_first.size();
+  for (int k = 0; k < n_slices; k++) {            // every slice repeats the header fields, dec_ref_pic_marking included
+    ss.first_mb = n_slices > 1 ? slice_first[k] : 0;
+    ss.end_mb = k + 1 < n_slices ? slice_first[k + 1] : -1;
+    rbsp.clear();
+    if (sp.entropy_cabac) write_slice_cabac(sp, ss, mbs, &rbsp);
+    else write_slice(sp, ss, mbs, &rbsp, record_mb_bits ? &last_mb_bits : nullptr);
+    append_nal(au, 3, idr ? 5 : 1, rbsp);
+  }
   frame_num = (frame_num + 1) & 0x7fff;
   frames_coded++;
   force_idr = false;

@@ -2,7 +2,7 @@
 // slice serialisation from the device's MbOut records.  Mirrors the small part of
 // codec/encoder/core/src/encoder_ext.cpp (WelsEncoderEncodeExt :3441, frame_num / idr_pic_id handling
 // :3131,:3253) that the supported configuration exercises: CAMERA_VIDEO_REAL_TIME, 1 spatial + 1
-// temporal layer, RC_OFF_MODE, SM_SINGLE_SLICE, CAVLC, 1 reference frame, IDR only at the start
+// temporal layer, RC_OFF_MODE, fixed slice partitions, CAVLC, 1 reference frame, IDR only at the start
 // (uiIntraPeriod = 0) or on ForceIntraFrame.
 #pragma once
 #include <vector>
@@ -54,11 +54,13 @@ struct StreamCtl {
 
   void init(int width, int height, int qp, float fps_, int target_bitrate, int entropy_cabac = 0, int profile_idc = 0);
   bool next_is_idr() const { return force_idr; }
+  // first macroblock of every slice of a picture (enc_slices.h: SliceConfig::starts), set before set_loop_filter; empty: one slice
+  std::vector<int32_t> slice_first;
   // iLoopFilterDisableIdc / iLoopFilterAlphaC0Offset / iLoopFilterBetaOffset (after init): with one slice per picture idc 2 is
   // idc 0 (encoder_ext.cpp:1109-1114); false if a value is out of range (encoder_ext.cpp:316-318)
   bool set_loop_filter(int idc, int alpha_c0_offset, int beta_offset) {
     if (idc < 0 || idc > 2 || alpha_c0_offset < -6 || alpha_c0_offset > 6 || beta_offset < -6 || beta_offset > 6) return false;
-    sp.dbk_idc = idc == 2 ? 0 : idc; sp.dbk_alpha_div2 = alpha_c0_offset; sp.dbk_beta_div2 = beta_offset;
+    sp.dbk_idc = idc == 2 && slice_first.size() < 2 ? 0 : idc; sp.dbk_alpha_div2 = alpha_c0_offset; sp.dbk_beta_div2 = beta_offset;
     return true;
   }
   // geometry of the padded pictures (PicLayout)
@@ -67,7 +69,7 @@ struct StreamCtl {
   int rec_rows_y() const { return PicLayout(sp.mb_w, sp.mb_h).rows_y; }
   int rec_rows_c() const { return PicLayout(sp.mb_w, sp.mb_h).rows_c; }
   EncFrameParams frame_params(bool idr, bool ref_is_p) const;
-  // serialises the access unit of the frame just coded (SPS+PPS+IDR slice, or P slice)
+  // serialises the access unit of the frame just coded (SPS+PPS+IDR slices, or P slices: one NAL unit per slice)
   void write_access_unit(bool idr, const MbOut* mbs, std::vector<uint8_t>* au);                 // one record per MB
   // compact form (k_pack_records): idx[mb] = offset of the macroblock's record in `packed` in 32-byte units, or -1 for P_SKIP;
   // refs: the picture's reference syntax (enc_refs.h), NULL for the one-reference stream's

@@ -112,7 +112,7 @@ typedef struct {
   int32_t dec_mode;                       // 1: decoder construct path (MbInfo::p16x16_mv carries slice / deblocking control)
   int32_t fast_mode;                      // iComplexityMode == LOW_COMPLEXITY: SAD mode costs, VAA-driven partition choice
                                           // (SetFastCodingFunc / WelsMdInterFinePartitionVaa, encoder_ext.cpp:2616,2688)
-  int32_t dbk_idc, dbk_off_a, dbk_off_b;  // encoder: disable_deblocking_filter_idc (0 / 1), FilterOffsetA / B (2 x the slice header's div2 values)
+  int32_t dbk_idc, dbk_off_a, dbk_off_b;  // encoder: disable_deblocking_filter_idc (0 / 1, 2 with several slices), FilterOffsetA / B (2 x the slice header's div2 values)
   int32_t dec_cqp_off;                    // decoder: chroma_qp_index_offset of the picture's PPS (both chroma planes)
 } EncFrameParams;
 
@@ -134,4 +134,6 @@ typedef struct {
   const DecMbAuxB* dec_aux_b;             // decoder: list-1 records of the picture's macroblocks (NULL unless the picture holds B slices)
   const uint8_t* prev_luma;               // fast mode: luma of the previous SOURCE picture (same layout as cur[0])
   int32_t* mb_bits;                       // optional (NULL = off): exact CAVLC bits of every macroblock (enc_cavlc_bits.cuh)
+  const int32_t* slice_first;             // encoder, several slices per picture: per macroblock, the address of its slice's first
+                                          // macroblock (enc_slices.h); NULL: one slice
 } EncFramePtrs;

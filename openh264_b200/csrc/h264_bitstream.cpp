@@ -188,7 +188,7 @@ inline int nc_of(int a, int b) {          // a/b = neighbour counts or -1 when u
 const uint8_t* cbp_me_table(bool intra) { return intra ? kCbpIntra : kCbpInter; }
 
 void write_slice_header(BitWriter& w, const StreamParams& sp, const SliceState& ss) {
-  w.ue(0);                               // first_mb_in_slice
+  w.ue((uint32_t)ss.first_mb);           // first_mb_in_slice
   w.ue(ss.idr ? 2 : 0);                  // slice_type: I / P
   w.ue((uint32_t)sp.pps_id);             // pic_parameter_set_id
   w.put(15, (uint32_t)ss.frame_num);
@@ -220,11 +220,11 @@ void write_slice(const StreamParams& sp, const SliceState& ss, const MbOut* cons
   write_slice_header(w, sp, ss);
 
   // ---- slice data ----
-  const int mbw = sp.mb_w, n = sp.mb_w * sp.mb_h;
+  const int mbw = sp.mb_w, n = sp.mb_w * sp.mb_h, first = ss.first_mb, end = ss.end_mb < 0 ? n : ss.end_mb;
   int skip_run = 0;
   int last_qp = ss.qp;
-  if (mb_bits) mb_bits->assign(n, 0);
-  for (int idx = 0; idx < n; idx++) {
+  if (mb_bits) { mb_bits->resize(n); for (int idx = first; idx < end; idx++) (*mb_bits)[idx] = 0; }
+  for (int idx = first; idx < end; idx++) {
     const MbOut& m = *recs[idx];
     const int mbx = idx % mbw, mby = idx / mbw;
     if (m.mb_type == MBT_PSKIP) { skip_run++; continue; }
@@ -261,8 +261,8 @@ void write_slice(const StreamParams& sp, const SliceState& ss, const MbOut* cons
       w.se(m.qp - last_qp);
       last_qp = m.qp;
       // neighbour counts
-      const int8_t* L = mbx > 0 ? recs[idx - 1]->nnz : nullptr;
-      const int8_t* T = mby > 0 ? recs[idx - mbw]->nnz : nullptr;
+      const int8_t* L = mbx > 0 && idx - 1 >= first ? recs[idx - 1]->nnz : nullptr;
+      const int8_t* T = mby > 0 && idx - mbw >= first ? recs[idx - mbw]->nnz : nullptr;
       auto luma_nc = [&](int bx, int by) {
         const int a = bx > 0 ? m.nnz[by * 4 + bx - 1] : (L ? L[by * 4 + 3] : -1);
         const int b = by > 0 ? m.nnz[(by - 1) * 4 + bx] : (T ? T[12 + bx] : -1);

@@ -74,19 +74,20 @@ struct SliceState {
   bool long_term_reference_flag = false;  // IDR
   int n_mmco = 0;                       // P: adaptive_ref_pic_marking_mode_flag = n_mmco > 0
   int mmco[3][3] = {};                  // operation and its values, in the order they are written
+  int first_mb = 0, end_mb = -1;        // the slice's macroblocks [first_mb, end_mb) (raster run; -1: to the picture's end)
 };
 // slice header up to slice_beta_offset_div2 (svc_encode_slice.cpp:275-346); both entropy modes write it
 void write_slice_header(BitWriter& w, const StreamParams& sp, const SliceState& ss);
-// slice header + all macroblocks + trailing bits of a single-slice picture
 // coded_block_pattern me(v) mapping (Rec. H.264 Table 9-4, chroma_format_idc 1): codeNum indexed by cbp (48 entries)
 const uint8_t* cbp_me_table(bool intra);
 
-// recs[i] = the record of macroblock i (P_SKIP macroblocks may all point at one shared all-zero-nnz record)
-// mb_bits (optional): bits of macroblock_layer() of every macroblock (0 for P_SKIP; mb_skip_run not included)
+// slice header + the slice's macroblocks (ss.first_mb .. ss.end_mb) + trailing bits.  A neighbour outside the slice is not
+// available.  recs[i] = the record of macroblock i of the picture (P_SKIP macroblocks may all point at one shared all-zero-nnz record)
+// mb_bits (optional, sized to the picture): bits of macroblock_layer() of the slice's macroblocks (0 for P_SKIP; mb_skip_run not included)
 void write_slice(const StreamParams& sp, const SliceState& ss, const MbOut* const* recs, std::vector<uint8_t>* rbsp,
                  std::vector<int32_t>* mb_bits = nullptr);
 
-// the same picture through CABAC (entropy_coding_mode_flag = 1): h264_cabac.cpp
+// the same slice through CABAC (entropy_coding_mode_flag = 1; contexts initialised per slice): h264_cabac.cpp
 void write_slice_cabac(const StreamParams& sp, const SliceState& ss, const MbOut* const* recs, std::vector<uint8_t>* rbsp);
 
 }  // namespace b2h264

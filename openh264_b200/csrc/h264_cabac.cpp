@@ -178,17 +178,17 @@ void write_slice_cabac(const StreamParams& sp, const SliceState& ss, const MbOut
   CabacEncoder e(rbsp);                  // the header is byte aligned: the arithmetic coder appends whole bytes
   e.init_contexts(ss.qp, ss.idr ? 0 : 1);
 
-  const int mbw = sp.mb_w, n = sp.mb_w * sp.mb_h;
-  std::vector<MbCtxInfo> info((size_t)n);
+  const int mbw = sp.mb_w, first = ss.first_mb, end = ss.end_mb < 0 ? sp.mb_w * sp.mb_h : ss.end_mb;
+  std::vector<MbCtxInfo> info((size_t)(end - first));   // of the slice's macroblocks: a neighbour outside the slice is not available
   int last_qp = ss.qp;
   bool prev_dqp_nonzero = false;          // mb_qp_delta != 0 of the previous macroblock in decoding order (that carried one)
-  for (int idx = 0; idx < n; idx++) {
+  for (int idx = first; idx < end; idx++) {
     const MbOut& m = *recs[idx];
     const int mbx = idx % mbw, mby = idx / mbw;
-    const MbCtxInfo* L = mbx > 0 ? &info[idx - 1] : nullptr;
-    const MbCtxInfo* T = mby > 0 ? &info[idx - mbw] : nullptr;
-    MbCtxInfo& me = info[idx];
-    if (idx > 0) e.terminate(0);          // end_of_slice_flag of the previous macroblock
+    const MbCtxInfo* L = mbx > 0 && idx - 1 >= first ? &info[idx - 1 - first] : nullptr;
+    const MbCtxInfo* T = mby > 0 && idx - mbw >= first ? &info[idx - mbw - first] : nullptr;
+    MbCtxInfo& me = info[idx - first];
+    if (idx > first) e.terminate(0);      // end_of_slice_flag of the previous macroblock
 
     if (!ss.idr) e.decision(11 + (L && !L->skip ? 1 : 0) + (T && !T->skip ? 1 : 0), m.mb_type == MBT_PSKIP);   // mb_skip_flag
     if (m.mb_type == MBT_PSKIP) { me = MbCtxInfo(); prev_dqp_nonzero = false; continue; }

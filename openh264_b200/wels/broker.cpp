@@ -23,7 +23,16 @@ EncPool::EncPool(const PoolKey& key, int capacity, int device) : Batcher(capacit
   cfg.loop_filter_idc = key.dbk_idc; cfg.loop_filter_alpha_c0_offset = key.dbk_alpha; cfg.loop_filter_beta_offset = key.dbk_beta;
   if (b2h264_enc_create(&cfg, &enc_) != 0) { enc_ = nullptr; return; }
   // on failure ok() is false and the destructor releases what was acquired
-  if (b2h264_enc_set_references(enc_, key.num_ref_frames, key.ltr, 30) != 0 || cudaSetDevice(device) != cudaSuccess ||
+  // the resolved partition, handed back as a raster request that resolves to it: one slice per row (which a picture of at most
+  // 48 macroblocks keeps), or explicit runs
+  const int mb_w = (key.width + 15) >> 4, mb_h = (key.height + 15) >> 4;
+  bool rows = key.slice_num > 1 && key.slice_num == mb_h;
+  for (int k = 0; rows && k < key.slice_num; k++) rows = key.slice_mb[k] == (uint32_t)mb_w;
+  const uint32_t no_runs[b2h264::kMaxSlicesNum] = {};
+  if (b2h264_enc_set_references(enc_, key.num_ref_frames, key.ltr, 30) != 0 ||
+      b2h264_enc_set_slices(enc_, key.slice_num > 1 ? b2h264::kSmRaster : b2h264::kSmSingle, key.slice_num,
+                            rows ? no_runs : key.slice_mb) != 0 ||
+      cudaSetDevice(device) != cudaSuccess ||
       pinned_.alloc(frame_bytes_ * capacity, cudaHostAllocPortable) != cudaSuccess || d_stage_.alloc(frame_bytes_ * capacity) != cudaSuccess ||
       up_stream_.create(cudaStreamNonBlocking) != cudaSuccess) {
     b2h264_enc_destroy(enc_);

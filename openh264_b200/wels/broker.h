@@ -17,12 +17,14 @@
 //     already waiting (so a lone stream never waits).
 #pragma once
 #include <stdint.h>
+#include <string.h>
 
 #include <memory>
 #include <mutex>
 #include <vector>
 
 #include "../csrc/cuda_owned.h"
+#include "../csrc/enc_slices.h"
 #include "b2h264_codec.h"
 #include "batcher.h"
 
@@ -33,11 +35,15 @@ struct PoolKey {
   // resolved reference configuration (max_num_ref_frames of the SPS, LTR on / off): every stream of a pool has the same picture
   // store; the LTR marking period is per stream (EncPool::ltr_mark_period)
   int num_ref_frames = 1, ltr = 0;
+  // resolved slice partition (enc_slices.h): the run length of every slice; dbk_idc above is the idc as coded
+  int slice_num = 1;
+  uint32_t slice_mb[b2h264::kMaxSlicesNum] = {};
   float fps;
   bool operator==(const PoolKey& o) const {
     return width == o.width && height == o.height && qp == o.qp && bitrate == o.bitrate && strategy == o.strategy && complexity_low == o.complexity_low && entropy_cabac == o.entropy_cabac &&
            profile_idc == o.profile_idc && intra_period == o.intra_period && dbk_idc == o.dbk_idc &&
-           dbk_alpha == o.dbk_alpha && dbk_beta == o.dbk_beta && num_ref_frames == o.num_ref_frames && ltr == o.ltr && fps == o.fps;
+           dbk_alpha == o.dbk_alpha && dbk_beta == o.dbk_beta && num_ref_frames == o.num_ref_frames && ltr == o.ltr && fps == o.fps &&
+           slice_num == o.slice_num && memcmp(slice_mb, o.slice_mb, sizeof(slice_mb)) == 0;
   }
 };
 

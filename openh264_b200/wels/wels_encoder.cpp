@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "../csrc/enc_refs.h"
+#include "../csrc/enc_slices.h"
 #include "b2h264_codec.h"
 #include "broker.h"
 #include "codec_api.h"
@@ -65,7 +66,6 @@ class B2Encoder : public ISVCEncoder {
     REQUIRE(p->iUsageType == CAMERA_VIDEO_REAL_TIME, "iUsageType != CAMERA_VIDEO_REAL_TIME");
     REQUIRE(p->iSpatialLayerNum == 1 && p->iTemporalLayerNum == 1, "more than one spatial/temporal layer");
     REQUIRE(p->iRCMode == RC_OFF_MODE, "iRCMode != RC_OFF_MODE");
-    REQUIRE(l.sSliceArgument.uiSliceMode == SM_SINGLE_SLICE, "uiSliceMode != SM_SINGLE_SLICE");
     REQUIRE(p->iNumRefFrame == AUTO_REF_PIC_COUNT || (p->iNumRefFrame >= 1 && p->iNumRefFrame <= kMaxRefCamera),
             "iNumRefFrame outside 1..10 and not AUTO_REF_PIC_COUNT");
     if (p->iLoopFilterDisableIdc < 0 || p->iLoopFilterDisableIdc > 2 || p->iLoopFilterAlphaC0Offset < -6 || p->iLoopFilterAlphaC0Offset > 6 ||
@@ -88,6 +88,19 @@ class B2Encoder : public ISVCEncoder {
     REQUIRE((p->iPicWidth % 4) == 0 && (p->iPicHeight % 2) == 0, "width % 4 or height % 2");
     REQUIRE(l.iDLayerQp >= 0 && l.iDLayerQp <= 51, "iDLayerQp out of range");
     REQUIRE(p->uiMaxNalSize == 0, "uiMaxNalSize");
+    // the slice partition, resolved as the reference resolves it (enc_slices.h); refused where the reference's bytes would depend on
+    // the machine (load-balanced fixed slices, an automatic thread count) or on the bits spent (SM_SIZELIMITED_SLICE)
+    const SSliceArgument& sa = l.sSliceArgument;
+    b2h264::SliceConfig slices;
+    {
+      const char* reason = "uiSliceMode";
+      const int num = sa.uiSliceNum > 1000u ? 1000 : (int)sa.uiSliceNum;
+      REQUIRE(b2h264::SliceConfig::resolve((int)sa.uiSliceMode, num, sa.uiSliceMbNum, (p->iPicWidth + 15) >> 4, (p->iPicHeight + 15) >> 4,
+                                           &slices, &reason), reason);
+    }
+    REQUIRE(slices.reproducible(p->iMultipleThreadIdc, p->bUseLoadBalancing),
+            "several slices with iMultipleThreadIdc 0, or fixed slices with bUseLoadBalancing on as many threads as slices (the "
+            "reference moves the slice boundaries by measured coding times)");
 #undef REQUIRE
     Uninitialize();
     b2wels::PoolKey key;
@@ -108,7 +121,8 @@ class B2Encoder : public ISVCEncoder {
     // Baseline / Main / High counts as unspecified: encoder_ext.cpp:126-141,652-664)
     key.entropy_cabac = p->iEntropyCodingModeFlag != 0 ? 1 : 0;
     key.profile_idc = (int)l.uiProfileIdc;
-    key.dbk_idc = p->iLoopFilterDisableIdc; key.dbk_alpha = p->iLoopFilterAlphaC0Offset; key.dbk_beta = p->iLoopFilterBetaOffset;
+    key.dbk_idc = slices.loop_filter_idc(p->iLoopFilterDisableIdc, p->iMultipleThreadIdc);
+    key.dbk_alpha = p->iLoopFilterAlphaC0Offset; key.dbk_beta = p->iLoopFilterBetaOffset;
     key.intra_period = p->uiIntraPeriod == (unsigned int)-1 ? 0 : (int)p->uiIntraPeriod;       // param_svc.h:370-372 (GOP size 1: no rounding)
     // reference pictures, resolved as the reference resolves them (au_set.cpp:88-133; camera LTR always keeps LONG_TERM_REF_NUM = 2
     // long-term pictures whatever iLTRRefNum asks): the pool is keyed on what reaches the bitstream and the picture store.  The
@@ -119,6 +133,8 @@ class B2Encoder : public ISVCEncoder {
     const int period = rc.ltr_mark_period;
     key.num_ref_frames = rc.sps_num_ref_frames;
     key.ltr = rc.ltr ? 1 : 0;
+    key.slice_num = slices.slices();
+    if (key.slice_num > 1) memcpy(key.slice_mb, slices.mb_num, sizeof(key.slice_mb));
     pool_ = b2wels::Broker::get().attach(key, &slot_);
     if (!pool_ || slot_ < 0) { pool_.reset(); slot_ = -1; return cmMallocMemeError; }
     if (pool_->ltr_mark_period(slot_, period) != 0) { Uninitialize(); return cmInitParaError; }
@@ -127,6 +143,13 @@ class B2Encoder : public ISVCEncoder {
     // what GetOption(ENCODER_OPTION_SVC_ENCODE_PARAM_EXT) reports is the RESOLVED configuration, as with the reference
     // (param_svc.h:370-372, encoder_ext.cpp:126-141,652-664)
     if (par_.uiIntraPeriod == (unsigned int)-1) par_.uiIntraPeriod = 0;
+    if (sa.uiSliceMode != SM_SINGLE_SLICE) {
+      SSliceArgument& r = par_.sSpatialLayers[0].sSliceArgument;
+      r.uiSliceMode = (SliceModeEnum)slices.mode;
+      r.uiSliceNum = (unsigned int)slices.num;
+      for (int i = 0; i < b2h264::kMaxSlicesNum; i++) r.uiSliceMbNum[i] = slices.mb_num[i];
+      r.uiSliceSizeConstraint = 0;
+    }
     par_.bEnableAdaptiveQuant = false;
     {
       int32_t r[4];
@@ -290,8 +313,8 @@ class B2Encoder : public ISVCEncoder {
     }
   }
 
-  // The access unit is [SPS PPS] slice, each NAL behind a 4-byte start code.  The reference reports an IDR as
-  // two layers (parameter sets: NON_VIDEO_CODING_LAYER, then the slice: VIDEO_CODING_LAYER), a P picture as one.
+  // The access unit is [SPS PPS] slices, each NAL behind a 4-byte start code.  The reference reports an IDR as
+  // two layers (parameter sets: NON_VIDEO_CODING_LAYER, then the slices: VIDEO_CODING_LAYER), a P picture as one.
   void fill_info(SFrameBSInfo* info, bool idr, long long ts) {
     memset(info, 0, sizeof(*info));
     nal_len_.clear();
@@ -307,10 +330,10 @@ class B2Encoder : public ISVCEncoder {
       SLayerBSInfo& l = info->sLayerInfo[layer++];
       l.eFrameType = ft;
       l.uiLayerType = NON_VIDEO_CODING_LAYER;
-      l.iNalCount = (int)nal_len_.size() - 1;
+      l.iNalCount = 2;                                             // SPS, PPS
       l.pNalLengthInByte = nal_len_.data();
       l.pBsBuf = au_.data();
-      first_vcl = nal_len_.size() - 1;
+      first_vcl = 2;
     }
     SLayerBSInfo& v = info->sLayerInfo[layer++];
     v.eFrameType = ft;
